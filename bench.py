@@ -2,9 +2,9 @@
 """bench.py -- the headline metric of BASELINE.json on this repo's engine.
 
     metric : RAG queries/sec, 10M x 1536 bf16 corpus, top-10 (cosine), recall@10 vs numpy
-    step   : `batches_per_step` batches of `--batch` queries, each searched against the whole corpus
-             (VECTOR_SEARCH_AGG, reference call site terraform/lab2-vector-search/main.tf:292); the driver fixes
-             --steps, so a step holds as many batches as it takes to make the timed region >= 2 s (sustained clocks)
+    step   : one batch of `--batch` queries searched against the whole corpus (VECTOR_SEARCH_AGG, reference call
+             site terraform/lab2-vector-search/main.tf:292); the timed region is exactly `--steps` steps, after an
+             untimed preheat that brings the GPU to its sustained clocks
     value  : whole-job queries/sec with the queries already resident in HBM (CUDA events, max over ranks)
     e2e    : same metric through the host-buffer C-ABI calls (H2D of the fp32 queries and D2H of the results inside
              the timed region, two batches in flight): sa_search_host_submit/_wait at N = 1,
@@ -21,6 +21,9 @@ source and what the CPU oracle reads: builder, judge and oracle see identical bi
 
 After the headline measurement the same process measures the other BASELINE.json configs (`extra_configs`: config 2,
 config 4's batch and config 5's shard shape with streaming epochs), each with its own recall check and roofline.
+
+`--dump-outputs DIR` writes what the last timed step returned (DIR/scores.npy float32, DIR/indices.npy float64, one
+row per query) so that two builds can be compared output for output: the inputs are seeded and identical run to run.
 
 `--impl reference` times the CPU arm instead: the numpy brute-force oracle (BASELINE.md section 4) with all host
 threads on a bounded sample of the same workload.  It never touches the GPU engine.
@@ -77,7 +80,9 @@ def parse_args():
     ap.add_argument("--recall-queries", type=int, default=256, help="queries checked against numpy over ALL rows")
     ap.add_argument("--cpu-sample-queries", type=int, default=256)
     ap.add_argument("--cpu-sample-rows", type=int, default=524_288)
-    ap.add_argument("--min-timed-s", type=float, default=2.0, help="minimum length of every timed region")
+    ap.add_argument("--min-timed-s", type=float, default=2.0, help="minimum length of the Avro pipeline's timed region")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write the last step's results (scores.npy float32, indices.npy float64)")
     ap.add_argument("--preheat-max", type=float, default=6.0,
                     help="untimed back-to-back searches until the SM clock has been stable for 1 s (at most this long), so "
                          "the timed steps run at the sustained (power-capped) clocks the sustained peak was measured at")
@@ -107,7 +112,8 @@ def measured_peaks():
             d = json.load(f)
         return {"hbm_gbs": d["hbm_gbs"], "tflops_burst": d["bf16_tflops"],
                 "tflops_sustained": d.get("bf16_tflops_sustained", d["bf16_tflops"]), "source": "measured"}
-    return {"hbm_gbs": 6650.0, "tflops_burst": 1590.0, "tflops_sustained": 1400.0, "source": "fallback"}
+    # H100 SXM data sheet (700 W part): HBM3 bandwidth and dense BF16 tensor rate -- ceilings, not measurements
+    return {"hbm_gbs": 3350.0, "tflops_burst": 989.0, "tflops_sustained": 989.0, "source": "H100 SXM data sheet"}
 
 
 # ----------------------------------------------------------------------------------------------------
@@ -460,14 +466,14 @@ def _all_reduce_max_list(vals, dist, torch):
     return t.tolist()
 
 
-def settle_and_estimate(step, sync, barrier, sampler, world, allmax, steps, min_timed_s, preheat_max, settle_s=1.5):
-    """Bring the GPU to its sustained state and size a step.  Returns (batches per step, preheat seconds, preheat batches,
-    seconds per batch).
+def settle_and_estimate(step, sync, barrier, sampler, world, allmax, preheat_max, settle_s=1.5):
+    """Bring the GPU to its sustained state and time a batch.  Returns (preheat seconds, preheat batches, seconds per
+    batch).
       1. one-time costs first (NCCL connection set-up, first-use allocations): they must not reach any estimate -- a first
          version let them in, took 0.3 s for a batch, and timed a 0.06 s region at boost clocks;
       2. preheat (untimed) until the SM clock is stable UNDER LOAD: a 1 kW part boosts for the first second and then
          settles at its power cap; the roofline denominator (cuBLAS, 4 s back to back) is a settled number;
-      3. seconds per batch from a short settled burst; a step = as many batches as make the timed region >= min_timed_s."""
+      3. seconds per batch from a short settled burst."""
     for _ in range(3):
         step()
     barrier()
@@ -485,8 +491,7 @@ def settle_and_estimate(step, sync, barrier, sampler, world, allmax, steps, min_
     est = (time.perf_counter() - t_e0) / 8
     if world > 1:
         est = allmax([est])[0]
-    inner = max(1, int(math.ceil(min_timed_s / max(steps * est, 1e-9))))
-    return inner, ph_s, n_ph, est
+    return ph_s, n_ph, est
 
 
 class Workload:
@@ -545,12 +550,13 @@ class Workload:
         env["barrier"]()
         return time.perf_counter() - t0, res
 
-    def measure(self, steps, warmup, min_timed_s, preheat_max, sampler):
+    def measure(self, steps, warmup, preheat_max, sampler):
         a, env = self.a, self.env
         torch = env["torch"]
         world = env["world"]
-        inner, ph_s, n_ph, est = settle_and_estimate(self.step_device, torch.cuda.synchronize, env["barrier"], sampler, world,
-                                                     env["allmax"], steps, min_timed_s, preheat_max)
+        ph_s, n_ph, est = settle_and_estimate(self.step_device, torch.cuda.synchronize, env["barrier"], sampler, world,
+                                              env["allmax"], preheat_max)
+        inner = 1   # batches per step
         # ---- warm-up steps
         for _ in range(warmup):
             out = self.step_device()
@@ -565,23 +571,17 @@ class Workload:
         for _ in range(warmup):   # back to back again: the timed device loop must not start from the e2e loop's tail
             out = self.step_device()
 
-        # ---- timed: device-resident queries, `steps` steps of `inner` batches.  Should the region come out shorter than
-        # asked for (a bad estimate), it is repeated once with the batch count the measurement itself implies.
+        # ---- timed: device-resident queries, exactly `steps` steps
         ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        for attempt in range(2):
-            env["barrier"]()
-            t_w0 = time.perf_counter()
-            ev0.record()
-            for _ in range(steps * inner):
-                out = self.step_device()
-            ev1.record()
-            env["barrier"]()
-            t_w1 = time.perf_counter()
-            ms_total = ev0.elapsed_time(ev1)
-            ms_max = env["allmax"]([ms_total])[0] if world > 1 else ms_total
-            if ms_max >= 0.6e3 * min_timed_s or attempt == 1:
-                break
-            inner = max(inner + 1, int(math.ceil(inner * min_timed_s * 1e3 / max(ms_max, 1e-3))))
+        env["barrier"]()
+        t_w0 = time.perf_counter()
+        ev0.record()
+        for _ in range(steps * inner):
+            out = self.step_device()
+        ev1.record()
+        env["barrier"]()
+        t_w1 = time.perf_counter()
+        ms_total = ev0.elapsed_time(ev1)
         t = self.ix.last_timing()
         # scan-kernel time: CUDA events recorded inside the C ABI on the launching stream around every scan launch of
         # the timed loop above (ring of the last 16 searches) -- back to back, no host synchronisation in between
@@ -618,16 +618,7 @@ class Workload:
         else:
             roof = {"bound": "hbm", "achieved": ach_gbs, "peak": peaks["hbm_gbs"], "unit": "GB/s",
                     "frac": ach_gbs / peaks["hbm_gbs"], "peak_kind": f"{peaks['source']} copy bandwidth"}
-        traffic = None
-        try:   # dram__bytes_read + write of this kernel from the committed `ncu --set full` capture of this workload
-            with open(os.path.join(ROOT, "profiles", "traffic.json")) as f:
-                tj = json.load(f).get(f"{n_local}x{dim}_b{B}_k{k}")
-            if tj:
-                traffic = tj["dram_bytes_per_launch"]
-                roof["traffic_source"] = tj["source"]
-        except Exception:
-            pass
-        roof.update({"traffic": traffic, "algorithmic_bytes": bytes_launch, "algorithmic_flops": flops_launch,
+        roof.update({"algorithmic_bytes": bytes_launch, "algorithmic_flops": flops_launch,
                      "kernel": "sa_scan_kernel", "launch_ms": t_launch * 1e3, "launches_per_batch": launches,
                      "launches_timed": n_timed * launches, "achieved_gbs": ach_gbs, "achieved_tflops": ach_tf,
                      "hbm_frac": ach_gbs / peaks["hbm_gbs"], "tensor_frac_sustained": ach_tf / peaks["tflops_sustained"],
@@ -689,6 +680,15 @@ class Workload:
         if world > 1:
             r["all_ranks_same_answer"] = bool(same.item())
         return r
+
+
+def dump_outputs(path, out):
+    """What the timed path returned to its caller in its last step: the top-k cosines (float32) and rows (float64,
+    exact), one row per query of the batch."""
+    os.makedirs(path, exist_ok=True)
+    scores, rows = (t.cpu().numpy() for t in out)
+    np.save(os.path.join(path, "scores.npy"), scores.astype(np.float32))
+    np.save(os.path.join(path, "indices.npy"), rows.astype(np.float64))
 
 
 def pipeline_e2e(env, index_like, n_total, dim, B, k, q_bits, est_batch_s, min_timed_s, check_rows=None):
@@ -848,7 +848,8 @@ def run_b200(a):
     n_total, dim, B, k = a.rows, a.dim, a.batch, a.k
     lo_row, hi_row = rank * n_total // world, (rank + 1) * n_total // world
     n_local = hi_row - lo_row
-    n5_total, dim5 = 50_000_000, 768
+    # config 5: 50M x 768 over all GPUs (76.8 GB); a single 80 GB H100 holds half of it
+    n5_total, dim5 = (50_000_000 if world > 1 else 25_000_000), 768
     lo5, hi5 = rank * n5_total // world, (rank + 1) * n5_total // world
     shared_bytes = n_local * dim * 2
     mem_avail = host_memory_available()
@@ -922,8 +923,10 @@ def run_b200(a):
     # ================================================================ headline
     wl = Workload(a, env, ix, sh, host, n_total, n_local, lo_row, dim, B, k, q_bits,
                   workload_name(n_total, dim, B, k))
-    m, out, res_host, ms_total, nb_total = wl.measure(a.steps, a.warmup, a.min_timed_s, a.preheat_max, sampler)
+    m, out, res_host, ms_total, nb_total = wl.measure(a.steps, a.warmup, a.preheat_max, sampler)
     result = None
+    if a.dump_outputs and rank == 0:
+        dump_outputs(a.dump_outputs, out)
     if rank == 0:
         data_note = (f"synthetic, canonical numpy PCG64 (oracle.synth_rows seed {a.seed} per 262144-row chunk, rows not "
                      f"pre-normalised; oracle.synth_queries seed {a.qseed}, odd queries planted next to rows of chunk 0)")
@@ -1006,7 +1009,7 @@ def run_b200(a):
             if world > 1:
                 raise   # ranks must not diverge inside collectives
 
-    ex_steps, ex_min_s, ex_ph = max(4, min(a.steps, 10)), min(a.min_timed_s, 1.0), min(a.preheat_max, 2.0)
+    ex_steps, ex_ph = max(4, min(a.steps, 10)), min(a.preheat_max, 2.0)
 
     def finish(w, mm, o, rh, nrq):
         rec = None if a.no_cpu else w.recall(o, rh, nrq)
@@ -1023,7 +1026,7 @@ def run_b200(a):
             ix.lib.sa_corpus_reset(ix._h)
             ix.commit(0, n2)                                   # config 2 = the first 1M rows of the same canonical corpus
             w = Workload(a, env, ix, sh, host, n2, n2, 0, dim, 256, k, q_bits2, workload_name(n2, dim, 256, k))
-            mm, o, rh, _, _ = w.measure(ex_steps, a.warmup, ex_min_s, ex_ph, sampler)
+            mm, o, rh, _, _ = w.measure(ex_steps, a.warmup, ex_ph, sampler)
             r = finish(w, mm, o, rh, 64)
             ix.lib.sa_corpus_reset(ix._h)
             ix.commit(0, n_local)
@@ -1033,7 +1036,7 @@ def run_b200(a):
         def cfg4():
             w = Workload(a, env, ix, sh, host, n_total, n_local, lo_row, dim, 4096, k, q_bits4,
                          workload_name(n_total, dim, 4096, k))
-            mm, o, rh, _, _ = w.measure(ex_steps, a.warmup, ex_min_s, ex_ph, sampler)
+            mm, o, rh, _, _ = w.measure(ex_steps, a.warmup, ex_ph, sampler)
             return finish(w, mm, o, rh, 64 if world == 1 else 32)
         run_extra("cfg4_10Mx1536_b4096", cfg4)
     if "cfg5" in extras:
@@ -1041,7 +1044,7 @@ def run_b200(a):
             nonlocal ix, sh
             sh.close()
             ix.close()
-            wl.ix = wl.sh = ix = sh = None                      # drop the 10M-row shard before the 50M x 768 one is built
+            wl.ix = wl.sh = ix = sh = None                      # drop the 10M-row shard before the config-5 one is built
             torch.cuda.empty_cache()
             n5 = hi5 - lo5
             ix5 = VectorIndex(dim=dim5, capacity=n5, max_batch=128, max_k=5, device=local)
@@ -1050,7 +1053,7 @@ def run_b200(a):
             q5 = bcast_queries(8765, 128, dim5, c0)
             sh5 = ShardedIndex(ix5, row_offset=lo5)
             w = Workload(a, env, ix5, sh5, host, n5_total, n5, lo5, dim5, 128, 5, q5, workload_name(n5_total, dim5, 128, 5))
-            mm, o, rh, _, _ = w.measure(ex_steps, a.warmup, ex_min_s, ex_ph, sampler)
+            mm, o, rh, _, _ = w.measure(ex_steps, a.warmup, ex_ph, sampler)
             r = finish(w, mm, o, rh, 32)
             # streaming form (BASELINE config 5: "appended in 1M-row epochs"): start with the last 8 epochs uncommitted,
             # publish one epoch (1M rows over all GPUs) every 4 batches while searching; final state == the full corpus
@@ -1083,7 +1086,7 @@ def run_b200(a):
             sh5.close()
             ix5.close()
             return r
-        run_extra("cfg5_50Mx768_b128_k5", cfg5)
+        run_extra(f"cfg5_{n5_total // 1_000_000}Mx768_b128_k5", cfg5)
 
     sampler.stop()
     host.close()

@@ -1,4 +1,4 @@
-/* sa_api.h -- C ABI of the B200-native vector-search engine (libsa_b200.so).
+/* sa_api.h -- C ABI of the H100-native vector-search engine (libsa_b200.so).
  *
  * This is the drop-in boundary for the one data-parallel path of confluentinc/quickstart-streaming-agents:
  * the Lab2 RAG lookup that the reference runs as Flink SQL inside Confluent Cloud against a MongoDB Atlas
@@ -14,7 +14,7 @@
  *   - `stream` is a cudaStream_t passed as an integer (0 = the legacy default stream); device entry points
  *     are asynchronous on it, *_host entry points block until their result is in host memory;
  *   - an engine serves one CUDA device and is not re-entrant;
- *   - there is no CPU fallback: on a device that is not sm_100 sa_engine_create fails with SA_ERR_DEVICE.
+ *   - there is no CPU fallback: on a device that is not sm_90 sa_engine_create fails with SA_ERR_DEVICE.
  */
 #ifndef SA_API_H_
 #define SA_API_H_

@@ -1,4 +1,4 @@
-"""B200-native vector search for the Lab2 RAG path of confluentinc/quickstart-streaming-agents.
+"""H100-native vector search for the Lab2 RAG path of confluentinc/quickstart-streaming-agents.
 
 Import as ``qsa_b200`` (see qsa_b200/__init__.py).  Modules:
   capi      ctypes binding of libsa_b200.so (include/sa_api.h)

@@ -59,7 +59,7 @@ def load() -> C.CDLL:
     if not os.path.exists(LIB_PATH):
         raise SaLibraryMissing(
             f"{LIB_PATH} not found: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-            "(nvcc, sm_100a). There is no CPU fallback.")
+            "(nvcc, sm_90a). There is no CPU fallback.")
     lib = C.CDLL(LIB_PATH)
     vp, i32, i64, u64, f32p = C.c_void_p, C.c_int, C.c_int64, C.c_uint64, C.POINTER(C.c_float)
     sig = {

@@ -99,8 +99,8 @@ struct DeviceGuard {
   if (_dg.rc != cudaSuccess) return fail(SA_ERR_CUDA, "cudaSetDevice(%d) failed: %s", (dev), cudaGetErrorString(_dg.rc))
 
 constexpr int kMaxLaunches = 16;
-constexpr int kDefaultWaitHintNs = 0;  // set from tools/gpu_sweep.py --opt wait_hint_ns=... (profiles/)
-constexpr int kDefaultPresample = 0;   // set from tools/gpu_worstcase.py / gpu_sweep.py (profiles/)
+constexpr int kDefaultWaitHintNs = 0;  // plain polling (option "wait_hint_ns" overrides)
+constexpr int kDefaultPresample = 0;   // no sampling pre-pass (option "presample" overrides)
 constexpr int kTimingRing = 16;
 constexpr int kHostSlots = SA_HOST_SLOTS;
 
@@ -117,7 +117,7 @@ struct sa_engine {
   uint16_t* corpus = nullptr;  // caller-owned
   float* inv_norm = nullptr;   // caller-owned
   int64_t n_rows = 0;
-  CUtensorMap tmap_c[2];       // [0]: box 256 rows (cta_group 1), [1]: box 128 rows (cta_group 2)
+  CUtensorMap tmap_c[2];       // [0]: box 128 rows (cta_group 1), [1]: box 64 rows (cta_group 2, multicast)
   bool bound = false;
 
   // scratch (library-owned)
@@ -309,8 +309,8 @@ int launch_scan_dispatch(int cg, int kl, int mode, const CUtensorMap& tq, const 
 
 int choose_cg(const sa_engine* e, int nq) {
   if (e->opt_cta_group == 1 || e->opt_cta_group == 2) return e->opt_cta_group;
-  // Auto: a CTA pair shares the corpus tile between two query blocks (half the smem/L2 operand traffic per
-  // flop), which pays once the batch fills 256-row pair blocks; small batches are HBM-bound and use 1 CTA.
+  // Auto: a CTA pair shares the corpus tile between two query blocks (each corpus slice is read from L2 once and
+  // multicast to both), which pays once the batch fills 256-row pair blocks; small batches are HBM-bound and use 1 CTA.
   return nq > 128 ? 2 : 1;
 }
 
@@ -406,9 +406,8 @@ int do_search(sa_engine* e, const uint16_t* q_bf16, int nq, int k, float* out_sc
     sp.max_drift = e->opt_max_drift >= 0 ? e->opt_max_drift : 1;
     sp.pace_gain = 0;
     sp.unit_map = e->opt_unit_map;
-    // drift-control defaults: round 1 tuned them on DRAM bytes (pairs 16 cycles per tile of lead beyond 1 tile); re-tuned
-    // on scan time after the epilogue rewrite (profiles/r02_sweep_drift_control.json, B = 1024: no pacing 28.8 ms,
-    // gain 16 -> 26.2, 32 -> 25.9, 64 -> 25.75; max_drift 0 / 2 no better than 1)
+    // drift-control defaults: one tile of free lead, then 32 (single CTAs) or 64 (pairs) cycles of delay per K-slice
+    // issue per extra tile of lead; options "max_drift", "pace_gain" and "pace_max" override them
     const int gain = e->opt_pace_gain >= 0 ? e->opt_pace_gain : (lp.cg == 2 ? 64 : 32);
     sp.pace_max = e->opt_pace_max >= 0 ? e->opt_pace_max : 8 * gain;
     if (lp.nqb > 1 && gain > 0) {
@@ -435,7 +434,7 @@ int do_search(sa_engine* e, const uint16_t* q_bf16, int nq, int k, float* out_sc
       // Sampling pre-pass: the same kernel over every presample-th tile, then each query's kKL-th best of the sample
       // becomes its shared threshold (a valid lower bound on its global kKL-th best).  The full scan then starts with
       // thresholds near their final values whatever the order of the rows: an adversarial (e.g. ascending) order can no
-      // longer make every row an insertion (tools/gpu_worstcase.py).
+      // longer make every row an insertion.
       sa::ScanParams pp = sp;
       pp.tile_stride = presample;
       pp.lane_progress = nullptr;  // no pacing: the pre-pass is short
@@ -594,7 +593,7 @@ const char* sa_strerror(int rc) {
     case SA_ERR_ARG: return "bad argument";
     case SA_ERR_COMM: return "collective error";
     case SA_ERR_CAPACITY: return "capacity exceeded";
-    case SA_ERR_DEVICE: return "unsupported device (needs compute capability 10.x / sm_100a)";
+    case SA_ERR_DEVICE: return "unsupported device (needs compute capability 9.0 / sm_90a)";
     default: return "unknown status";
   }
 }
@@ -614,8 +613,8 @@ int sa_engine_create(sa_engine** out, int device, int dim, int64_t capacity_rows
   if (device < 0 || device >= ndev) return fail(SA_ERR_ARG, "device %d not present (%d devices)", device, ndev);
   cudaDeviceProp prop;
   SA_CUDA(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10)
-    return fail(SA_ERR_DEVICE, "device %d is sm_%d%d; this library contains sm_100a code only", device, prop.major,
+  if (prop.major != 9 || prop.minor != 0)
+    return fail(SA_ERR_DEVICE, "device %d is sm_%d%d; this library contains sm_90a code only", device, prop.major,
                 prop.minor);
   SA_ON_DEVICE(device);
   if (!get_encode_fn()) return fail(SA_ERR_CUDA, "cuTensorMapEncodeTiled entry point not available");
@@ -743,9 +742,11 @@ int sa_corpus_bind(sa_engine* e, void* rows_bf16_dev, float* inv_norm_dev, int64
   if (reinterpret_cast<uintptr_t>(inv_norm_dev) % 16) return fail(SA_ERR_ARG, "inv_norm must be 16-byte aligned");
   if (n_valid < 0 || n_valid > e->capacity) return fail(SA_ERR_CAPACITY, "n_valid outside [0, capacity]");
   SA_ON_DEVICE(e->device);
-  int rc = encode_rows_map(&e->tmap_c[0], rows_bf16_dev, static_cast<uint64_t>(e->capacity), e->dim, sa::kBlockN);
+  int rc = encode_rows_map(&e->tmap_c[0], rows_bf16_dev, static_cast<uint64_t>(e->capacity), e->dim,
+                           sa::ScanCfg<1>::kBRows);
   if (rc) return rc;
-  rc = encode_rows_map(&e->tmap_c[1], rows_bf16_dev, static_cast<uint64_t>(e->capacity), e->dim, sa::kBlockN / 2);
+  rc = encode_rows_map(&e->tmap_c[1], rows_bf16_dev, static_cast<uint64_t>(e->capacity), e->dim,
+                       sa::ScanCfg<2>::kBRows);
   if (rc) return rc;
   e->corpus = static_cast<uint16_t*>(rows_bf16_dev);
   e->inv_norm = inv_norm_dev;

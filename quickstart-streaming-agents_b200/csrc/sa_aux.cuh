@@ -154,7 +154,7 @@ struct MergeParams {
 
 constexpr int kMergeThreads = 160;  // >= kMaxLanes: one thread per tile lane in the head tournament
 constexpr int kMergeWarps = kMergeThreads / 32;
-constexpr int kMaxLanes = 148;      // tile lanes of one scan launch (the planner caps TL here)
+constexpr int kMaxLanes = 132;      // tile lanes of one scan launch (the planner caps TL here): one per H100 SM
 constexpr int kSelMax = 128;        // candidates re-scored per query without the fallback
 
 __device__ __forceinline__ float key_score(unsigned long long k) {

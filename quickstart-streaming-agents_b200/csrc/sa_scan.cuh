@@ -1,17 +1,18 @@
 // The hot path: VECTOR_SEARCH_AGG(<corpus>, DESCRIPTOR(embedding), <query vector>, k)
 // (reference call sites: terraform/lab2-vector-search/main.tf:292, LAB3-Walkthrough.md:343-350,
-//  LAB4-Walkthrough.md:302-309) as one persistent, warp-specialised sm_100a kernel:
+//  LAB4-Walkthrough.md:302-309) as one persistent, warp-specialised sm_90a kernel:
 //
 //   TMA (SWIZZLE_128B tiles of the bf16 corpus and of the query block)  ->  smem ring
-//   tcgen05.mma  Q[128 x D] . C[256 x D]^T, fp32 accumulators in TMEM (two 256-column buffers)
-//   epilogue warps: tcgen05.ld -> scale by the row's 1/|c| -> per-thread (thread == query) sorted register list
+//   wgmma  Q[64 x D] . C[128 x D]^T per consumer warpgroup, fp32 accumulators in registers
+//   epilogue: accumulators -> smem -> scale by the row's 1/|c| -> per-thread (thread == query) sorted register list
 //
 // Nothing but the per-CTA candidate lists (kKL entries per query, plus one "dropped" bound per query) leaves the SM.
 //
-// Work decomposition.  A "unit" is one CTA (kCG == 1, 128-query blocks) or one CTA pair (kCG == 2, 256-query
-// blocks, tcgen05 cta_group::2).  Unit u owns query block qb = u % nqb and tile lane tl = u / nqb and walks corpus
-// tiles tl, tl + TL, tl + 2 TL, ... (256 rows each).  All units of one tile lane touch the same corpus tile at about
-// the same time (drift control below keeps it so): it crosses HBM once and is served from L2 to the others.
+// Work decomposition.  A "unit" is one CTA (kCG == 1, 128-query blocks) or a cluster of two CTAs (kCG == 2, 256-query
+// blocks: each CTA loads half of every corpus slice and multicasts it to both, so the pair reads each corpus tile once).
+// Unit u owns query block qb = u % nqb and tile lane tl = u / nqb and walks corpus tiles tl, tl + TL, tl + 2 TL, ...
+// (256 rows each, taken as two 128-row halves).  All units of one tile lane touch the same corpus tile at about the
+// same time (drift control below keeps it so): it crosses HBM once and is served from L2 to the others.
 //
 // Exactness contract with the merge kernel (sa_aux.cuh).  A thread's list holds the kKL best rows of its tile lane by
 // the scan's approximate score a = fp32_accumulate(q.c) * (1/|c|), and `drop` is an upper bound on the approximate
@@ -19,19 +20,20 @@
 // bound shared between lanes).  The merge kernel turns (lists, drops) into either a certificate that the exactly
 // re-scored candidates contain the true top-k, or a work item for the exact fallback scan.
 #pragma once
-#include "sm100_ptx.cuh"
+#include "sm90_ptx.cuh"
 #include <cmath>
 #include <cstring>
 
 namespace sa {
 
-constexpr int kBlockM = 128;  // queries per CTA  (TMEM lanes)
-constexpr int kBlockN = 256;  // corpus rows per tile (TMEM columns per accumulator)
+constexpr int kBlockM = 128;  // queries per CTA
+constexpr int kBlockN = 256;  // corpus rows per tile
+constexpr int kHalfN = kWgmmaN;  // corpus rows per MMA pass: a tile is scanned as two halves
 constexpr int kBlockK = 64;   // bf16 per K slice = 128 B = one swizzle atom
 constexpr int kUmmaK = 16;
-constexpr int kScanThreads = 256;  // w0 TMA, w1 MMA, w2 TMEM alloc, w3 idle, w4..7 epilogue
-constexpr int kTmemCols = 512;
-constexpr int kChunk = 32;         // TMEM columns per tcgen05.ld
+constexpr int kScanThreads = 384;  // warpgroup 0: w0 TMA producer; warpgroups 1, 2: 64 queries each (MMA + epilogue)
+constexpr int kChunk = 32;         // columns per list-update chunk
+constexpr int kStagingLd = kHalfN + 4;  // floats per query row of the accumulator staging buffer (conflict-free reads)
 constexpr int kWin = 16;           // tile lanes whose second-best scores an epilogue thread combines into a bound
 constexpr int kWinWarmTiles = 16;  // the window is read on every one of a lane's first tiles, later only after a slow one
 
@@ -42,24 +44,26 @@ constexpr int kModeProf = 2;   // profiling: per-role wait / busy cycle counters
 
 template <int kCG>
 struct ScanCfg {
-  static constexpr int kStages = (kCG == 1) ? 4 : 6;
-  static constexpr int kBRows = kBlockN / kCG;  // corpus rows staged by each CTA
+  static constexpr int kStages = 4;
+  static constexpr int kBRows = kHalfN / kCG;  // corpus rows of a half tile loaded (and multicast) by each CTA
   static constexpr uint32_t kABytes = kBlockM * kBlockK * 2;
-  static constexpr uint32_t kBBytes = kBRows * kBlockK * 2;
+  static constexpr uint32_t kBBytes = kHalfN * kBlockK * 2;  // what lands in each CTA per stage
   static constexpr uint32_t kStageBytes = kABytes + kBBytes;
+  static constexpr uint32_t kStagingBytes = kBlockM * kStagingLd * sizeof(float);
   static constexpr uint32_t kIcBytes = 4 * kBlockN * sizeof(float);  // one 256-float scale vector per epilogue warp
-  static constexpr uint32_t kBarBytes = (2 * kStages + 4) * 8 + 16;
+  static constexpr uint32_t kBarBytes = 2 * kStages * 8;
   // +1024: the dynamic smem base is aligned up to 1024 B by hand (SWIZZLE_128B requirement).
-  static constexpr uint32_t kSmemBytes = kStages * kStageBytes + kIcBytes + kBarBytes + 1024;
+  static constexpr uint32_t kSmemBytes = kStages * kStageBytes + kStagingBytes + kIcBytes + kBarBytes + 1024;
+  static_assert(kSmemBytes <= 227 * 1024, "H100 allows 227 KB of shared memory per block");
 };
 
 // Per-CTA profile record (kModeProf): SM cycles, summed over the kernel.
 struct ScanProf {
   long long prod_wait_empty;   // TMA producer blocked on a free smem slot
-  long long mma_wait_full;     // MMA issuer blocked on TMA data
-  long long mma_wait_tempty;   // MMA issuer blocked on the epilogue (accumulator not drained)
-  long long epi_wait_tfull;    // epilogue warp 0 blocked on the MMA (accumulator not complete)
-  long long epi_busy;          // epilogue warp 0 working on an accumulator
+  long long mma_wait_full;     // first consumer warpgroup blocked on TMA data
+  long long mma_wait_tempty;   // first consumer warpgroup blocked on its staging barriers (the other warps' epilogue)
+  long long epi_wait_tfull;    // first consumer warpgroup waiting for its last MMAs of a half tile to retire
+  long long epi_busy;          // first epilogue warp staging and scoring accumulators
   long long epi_slow_chunks;   // 32-column chunks of epilogue warp 0 that took the insertion path
   long long total;             // CTA lifetime
   long long tiles;             // tiles walked
@@ -78,7 +82,7 @@ struct ScanParams {
   float* part_drop;       // [gridDim.x][128]  upper bound on the approximate score of the lane's rows not in the list
   int corpus_evict_first; // 1: corpus tiles are read by a single query block -> stream them through L2
   int tile_stride;        // 1: walk every tile; S > 1: the sampling pre-pass walks tiles 0, S, 2S, ... only
-  int wait_hint_ns;       // suspend-time hint of the epilogue's mbarrier waits (0 = plain polling)
+  int wait_hint_ns;       // suspend-time hint of the consumers' mbarrier waits (0 = plain polling)
   int* lane_progress;     // [tl_count][nqb] tiles whose loads each unit has issued (zero at launch), or nullptr
   int unit_map;           // 0: unit = tl*nqb + qb (lane-mates adjacent), 1: unit = qb*TL + tl (lane-mates TL apart)
   int max_drift;          // lead (in tiles) over the slowest lane-mate that is not paced
@@ -244,9 +248,7 @@ struct TopList {
 // lowest row among equals), inserts it, masks it and re-reduces -- until nothing beats the threshold.  A warp executes
 // as many rounds as its busiest lane needs (usually one or two), however the qualifying values are spread over the 32
 // rows; walking the rows group by group instead costs a round per group that ANY lane has a hit in, which during the
-// warm-up of a short scan (1M rows: 26 tiles per lane) was most of the epilogue's time (A/B on B200,
-// profiles/r02_ab_insertion_walk.json: epilogue 15.1k -> 9.6k cycles per tile at 1M x 1536 / batch 256, scan +7..15 %;
-// 7.3k -> 4.6k at 6.25M x 768 / batch 128; neutral at batch 1024).
+// warm-up of a short scan (few tiles per lane) dominates the epilogue's time.
 template <int kKL>
 __host__ __device__ __forceinline__ bool chunk_process(TopList<kKL>& L, float (&v)[kChunk], const float (&w)[kChunk],
                                                        int row_base) {
@@ -295,57 +297,37 @@ __host__ __device__ __forceinline__ bool chunk_process(TopList<kKL>& L, float (&
 }
 
 #ifdef __CUDACC__
-// Epilogue of one accumulator: 256 columns of this thread's TMEM lane -> scaled scores -> list.
-// `ic` is this warp's private 256-float scale vector in shared memory (broadcast reads).
+// Epilogue of one half tile: 128 columns of this thread's query row in the staging buffer -> scaled scores -> list.
+// `ic` is this warp's private 256-float scale vector of the tile in shared memory (broadcast reads).
 template <int kKL, int kMode>
-__device__ __forceinline__ int epilogue_accumulator(TopList<kKL>& L, uint32_t taddr, const float* ic, int row0,
-                                                    float* dbg_row) {
-  L.apply_shared(L.nxt_key);
+__device__ __forceinline__ int epilogue_half(TopList<kKL>& L, const float* srow, const float* ic, int row0,
+                                             float* dbg_row) {
   int slow = 0;
-  float va[kChunk], vb[kChunk], w[kChunk];
-  const float4* ic4 = reinterpret_cast<const float4*>(ic);
-  auto load_w = [&](int c) {
+  float v[kChunk], w[kChunk];
+#pragma unroll 1
+  for (int c = 0; c < kHalfN / kChunk; ++c) {
+    const float4* s4 = reinterpret_cast<const float4*>(srow + c * kChunk);
+    const float4* w4 = reinterpret_cast<const float4*>(ic + c * kChunk);
 #pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const float4 x = ic4[c * 8 + i];
-      w[4 * i + 0] = x.x;
-      w[4 * i + 1] = x.y;
-      w[4 * i + 2] = x.z;
-      w[4 * i + 3] = x.w;
+    for (int i = 0; i < kChunk / 4; ++i) {
+      const float4 x = s4[i], y = w4[i];
+      v[4 * i + 0] = x.x;
+      v[4 * i + 1] = x.y;
+      v[4 * i + 2] = x.z;
+      v[4 * i + 3] = x.w;
+      w[4 * i + 0] = y.x;
+      w[4 * i + 1] = y.y;
+      w[4 * i + 2] = y.z;
+      w[4 * i + 3] = y.w;
     }
-  };
-  auto dump = [&](int c, const float (&v)[kChunk]) {
     if constexpr (kMode == kModeDots) {
       if (dbg_row != nullptr) {
 #pragma unroll
         for (int j = 0; j < kChunk; ++j) dbg_row[c * kChunk + j] = v[j];
       }
     }
-  };
-  __syncwarp();  // tcgen05.ld / wait::ld are .sync.aligned
-  tmem_ld_32x32(taddr, va);
-#pragma unroll 1
-  for (int c = 0; c < kBlockN / kChunk; c += 2) {
-    // chunk c is in flight into va: fetch its scales, wait, start chunk c+1 into vb, then work on va
-    load_w(c);
-    tmem_ld_wait(va);
-    tmem_ld_32x32(taddr + static_cast<uint32_t>((c + 1) * kChunk), vb);
-    dump(c, va);
-    slow += chunk_process<kKL>(L, va, w, row0 + c * kChunk) ? 1 : 0;
+    slow += chunk_process<kKL>(L, v, w, row0 + c * kChunk) ? 1 : 0;
     __syncwarp();  // reconverge after the divergent insertion path
-    load_w(c + 1);
-    tmem_ld_wait(vb);
-    if (c + 2 < kBlockN / kChunk) tmem_ld_32x32(taddr + static_cast<uint32_t>((c + 2) * kChunk), va);
-    dump(c + 1, vb);
-    slow += chunk_process<kKL>(L, vb, w, row0 + (c + 1) * kChunk) ? 1 : 0;
-    __syncwarp();
-  }
-  if (L.slot != nullptr) {
-    if (L.sc[kKL - 1] > L.published) {  // list full and its tail improved: tell the other lanes
-      L.published = L.sc[kKL - 1];
-      atomicMax(L.slot, float_to_key(L.published));
-    }
-    L.nxt_key = ld_relaxed_gpu_u32(L.slot);  // consumed at the start of the next accumulator: latency hidden
   }
   return slow;
 }
@@ -363,14 +345,11 @@ sa_scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t* smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
 
-  float* icbuf = reinterpret_cast<float*>(smem_gen + kStages * Cfg::kStageBytes);  // [4 warps][256]
-  const uint32_t bar_base = smem_base + kStages * Cfg::kStageBytes + Cfg::kIcBytes;
+  float* staging = reinterpret_cast<float*>(smem_gen + kStages * Cfg::kStageBytes);  // [128 queries][kStagingLd]
+  float* icbuf = reinterpret_cast<float*>(smem_gen + kStages * Cfg::kStageBytes + Cfg::kStagingBytes);  // [4][256]
+  const uint32_t bar_base = smem_base + kStages * Cfg::kStageBytes + Cfg::kStagingBytes + Cfg::kIcBytes;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (kStages + s); };
-  auto tfull_bar = [&](int a) { return bar_base + 8u * (2 * kStages + a); };
-  auto tempty_bar = [&](int a) { return bar_base + 8u * (2 * kStages + 2 + a); };
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem_gen + kStages * Cfg::kStageBytes + Cfg::kIcBytes +
-                                                    (2 * kStages + 4) * 8);
   auto a_smem = [&](int s) { return smem_base + s * Cfg::kStageBytes; };
   auto b_smem = [&](int s) { return smem_base + s * Cfg::kStageBytes + Cfg::kABytes; };
 
@@ -394,24 +373,13 @@ sa_scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant
   }
   if (warp == 1 && lane == 0) {
     for (int s = 0; s < kStages; ++s) {
-      mbar_init(full_bar(s), 1);   // the (leader) producer's arrive.expect_tx; TMA bytes complete it
-      mbar_init(empty_bar(s), 1);  // one tcgen05.commit per use
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(tfull_bar(a), 1);         // tcgen05.commit after an accumulator's last MMA
-      mbar_init(tempty_bar(a), 4 * kCG);  // one arrive per epilogue warp (of both CTAs of a pair)
+      mbar_init(full_bar(s), 1);         // this CTA producer's arrive.expect_tx; TMA bytes complete it
+      mbar_init(empty_bar(s), 2 * kCG);  // one arrive per consumer warpgroup of every CTA the slot is multicast to
     }
     fence_mbar_init();
   }
-  if (warp == 2) {
-    tmem_alloc<kCG>(smem_u32(tmem_slot), kTmemCols);
-    tmem_relinquish<kCG>();
-  }
-  tc_fence_before();
   __syncthreads();
-  if constexpr (kCG == 2) cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  if constexpr (kCG == 2) cluster_sync_all();  // the peer's barriers are initialised before any multicast or remote arrive
 
   // ------------------------------------------------------------------ roles
   if (warp == 0) {
@@ -422,9 +390,8 @@ sa_scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant
       uint32_t phase = 0;
       long long waited = 0;
       // Drift control between the units of a tile lane.  Units that share a corpus tile run identical work but at
-      // slightly different speeds (measured: ~3 % spread), so over thousands of tiles they drift tens of tiles
-      // apart; once the spread exceeds what L2 holds, every unit re-reads its tiles from HBM (measured 3.05x the
-      // algorithmic bytes at B = 1024).  A hard barrier costs a pipeline drain per tile (measured +20 %), so the
+      // slightly different speeds, so over thousands of tiles they drift tens of tiles apart; once the spread exceeds
+      // what L2 holds, every unit re-reads its tiles from HBM.  A hard barrier costs a pipeline drain per tile, so the
       // leader producers *pace* themselves instead: each publishes how many tiles it has issued, reads its
       // lane-mates' counters once per tile, and a unit that leads the slowest mate by more than `max_drift` tiles
       // delays every K-slice issue by pace_gain cycles per extra tile of lead (capped).  The kernel's duration is
@@ -442,32 +409,32 @@ sa_scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant
           for (int j = 0; j < nqb; ++j) slowest = min(slowest, ld_relaxed_gpu(pr + j));
           pace = min(max(tile_no - slowest - p.max_drift, 0) * p.pace_gain, p.pace_max);
         }
-        for (int kb = 0; kb < p.num_kb; ++kb) {
-          if constexpr (kProf) {
-            const long long c0 = clock64();
-            mbar_wait(empty_bar(stage), phase ^ 1u);
-            waited += clock64() - c0;
-          } else {
-            mbar_wait(empty_bar(stage), phase ^ 1u);
-          }
-          if (pace > 0) {
-            const long long c0 = clock64();
-            while (clock64() - c0 < pace) {
+        for (int h = 0; h < 2; ++h) {
+          for (int kb = 0; kb < p.num_kb; ++kb) {
+            if constexpr (kProf) {
+              const long long c0 = clock64();
+              mbar_wait(empty_bar(stage), phase ^ 1u);
+              waited += clock64() - c0;
+            } else {
+              mbar_wait(empty_bar(stage), phase ^ 1u);  // consumers of every CTA sharing the slot have released it
             }
-          }
-          if constexpr (kCG == 1) {
+            if (pace > 0) {
+              const long long c0 = clock64();
+              while (clock64() - c0 < pace) {
+              }
+            }
             mbar_expect_tx(full_bar(stage), Cfg::kStageBytes);
             tma_load_2d(a_smem(stage), &tmap_q, full_bar(stage), kb * kBlockK, q_row, kEvictLast);
-            tma_load_2d(b_smem(stage), &tmap_c, full_bar(stage), kb * kBlockK, t * kBlockN, c_hint);
-          } else {
-            if (rank == 0) mbar_expect_tx(full_bar(stage), 2 * Cfg::kStageBytes);
-            tma_load_2d_pair(a_smem(stage), &tmap_q, full_bar(stage), kb * kBlockK, q_row, kEvictLast);
-            tma_load_2d_pair(b_smem(stage), &tmap_c, full_bar(stage), kb * kBlockK,
-                             t * kBlockN + static_cast<int>(rank) * Cfg::kBRows, c_hint);
-          }
-          if (++stage == kStages) {
-            stage = 0;
-            phase ^= 1u;
+            const int c_row = t * kBlockN + h * kHalfN + static_cast<int>(rank) * Cfg::kBRows;
+            const uint32_t b_dst = b_smem(stage) + rank * (Cfg::kBRows * kBlockK * 2);
+            if constexpr (kCG == 1)
+              tma_load_2d(b_dst, &tmap_c, full_bar(stage), kb * kBlockK, c_row, c_hint);
+            else
+              tma_load_2d_multicast(b_dst, &tmap_c, full_bar(stage), kb * kBlockK, c_row, 0x3, c_hint);
+            if (++stage == kStages) {
+              stage = 0;
+              phase ^= 1u;
+            }
           }
         }
         if (lockstep) st_relaxed_gpu(p.lane_progress + tl * nqb + qb, tile_no + 1);
@@ -477,70 +444,29 @@ sa_scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant
         p.prof[blockIdx.x].tiles = tile_no;
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0 && rank == 0) {
-      // ===== MMA issuer (leader CTA of a pair) =====
-      constexpr uint32_t idesc = make_idesc_bf16_f32(kBlockM * kCG, kBlockN);
-      int stage = 0;
-      uint32_t phase = 0;
-      int it = 0;
-      long long w_full = 0, w_tempty = 0;
-      for (int ti = tl; ti < walk_tiles; ti += TL, ++it) {
-        const int a = it & 1;
-        const uint32_t aph = (it >> 1) & 1u;
-        if constexpr (kProf) {
-          const long long c0 = clock64();
-          mbar_wait(tempty_bar(a), aph ^ 1u);
-          w_tempty += clock64() - c0;
-        } else {
-          mbar_wait(tempty_bar(a), aph ^ 1u);  // epilogue has drained this accumulator
-        }
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + static_cast<uint32_t>(a * kBlockN);
-        for (int kb = 0; kb < p.num_kb; ++kb) {
-          if constexpr (kProf) {
-            const long long c0 = clock64();
-            mbar_wait(full_bar(stage), phase);
-            w_full += clock64() - c0;
-          } else {
-            mbar_wait(full_bar(stage), phase);
-          }
-          tc_fence_after();
-          const uint64_t a_desc = make_kmajor_sw128_desc(a_smem(stage));
-          const uint64_t b_desc = make_kmajor_sw128_desc(b_smem(stage));
-#pragma unroll
-          for (int k = 0; k < kBlockK / kUmmaK; ++k) {
-            // +32 B along K inside the 128-B swizzle atom = +2 in the (addr >> 4) field
-            umma_bf16<kCG>(d_tmem, a_desc + 2u * k, b_desc + 2u * k, idesc, (kb | k) != 0 ? 1u : 0u);
-          }
-          umma_commit<kCG>(empty_bar(stage));  // frees the smem slot (in both CTAs) once these MMAs retire
-          if (++stage == kStages) {
-            stage = 0;
-            phase ^= 1u;
-          }
-        }
-        umma_commit<kCG>(tfull_bar(a));  // accumulator complete -> epilogue
-      }
-      if constexpr (kProf) {
-        p.prof[blockIdx.x].mma_wait_full = w_full;
-        p.prof[blockIdx.x].mma_wait_tempty = w_tempty;
-      }
-    }
   } else if (warp >= 4) {
-    // ===== epilogue: thread == query row; 4 warps cover the 128 TMEM lanes; the warps never synchronise with each
-    // other (each stages its own copy of the tile's 256 scales), only with the MMA issuer through the mbarriers =====
-    const int ew = warp - 4;  // == warp % 4: the TMEM lane quarter this warp may read
-    const int et = ew * 32 + lane;
+    // ===== consumers: warpgroup g (1 or 2) multiplies queries [64 (g-1), 64 g) of the block with each half tile, stages
+    // the accumulators in smem, and its first two warps (thread == query) feed them to the candidate lists.  The two
+    // warpgroups only meet at the smem ring's barriers. =====
+    const int g = warp / 4 - 1;
+    const int wt = threadIdx.x & 127;          // thread within the warpgroup
+    const bool epi = (warp & 3) < 2;           // epilogue warp: its 32 lanes own 32 of the warpgroup's 64 queries
+    const int ew = 2 * g + (warp & 3);         // epilogue warp index within the CTA (valid when epi)
+    const int et = 64 * g + wt;                // query row within the CTA's block (valid when epi)
+    const bool signaller = wt == 0;            // releases smem slots and keeps the profile counters
+    const uint32_t named_bar = 1 + g;
     float* ic = icbuf + ew * kBlockN;
+    float* stg = staging + 64 * g * kStagingLd;
     // Threshold sharing.  A thread's list only ever sees its own tile lane, so alone it needs ~kKL*ln(n) insertions
     // to warm up, and a warp pays for every lane's insertions.  But if ANY lane already holds kKL rows scoring >= x
     // for this query, no row scoring < x can be in the query's global top-kKL.  So each epilogue thread publishes its
-    // kKL-th best (atomicMax on an order-preserving key) and reads the shared bound once per accumulator: every lane
-    // gets the threshold of the whole machine's progress, and the warm-up tail disappears.  The shared bound admits
-    // ties (>=), the thread's own bound stays strict (>), so tie-breaking by row is unchanged.
+    // kKL-th best (atomicMax on an order-preserving key) and reads the shared bound once per tile: every lane gets the
+    // threshold of the whole machine's progress, and the warm-up tail disappears.  The shared bound admits ties (>=),
+    // the thread's own bound stays strict (>), so tie-breaking by row is unchanged.
     const int query = qb * kRowsPerQb + static_cast<int>(rank) * kBlockM + et;
+    const bool own_query = epi && query < p.nq;
     TopList<kKL> L;
-    L.init((p.thr_shared != nullptr && query < p.nq) ? p.thr_shared + query : nullptr);
+    L.init((p.thr_shared != nullptr && own_query) ? p.thr_shared + query : nullptr);
 
     // Scales of tile t: lane l fetches rows [8l, 8l+8) (two 16-byte loads), masks rows past the committed prefix
     // and all-zero rows with NaN (NaN never compares greater than a threshold, so they cannot enter a list and
@@ -560,83 +486,145 @@ sa_scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant
         nx1 = make_float4(x[4], x[5], x[6], x[7]);
       }
     };
-    if (tl < walk_tiles) fetch_ic(tl * p.tile_stride);
+    if (epi && tl < walk_tiles) fetch_ic(tl * p.tile_stride);
 
     // Window bound (see window_bound): this thread's slot in the lanes' second-best table, and the kWin lanes it reads.
-    const bool win_on = p.lane2 != nullptr && TL >= kWin && query < p.nq;
+    const bool win_on = p.lane2 != nullptr && TL >= kWin && own_query;
     const size_t win_stride = static_cast<size_t>(p.nqb) * kRowsPerQb;
     unsigned* const win_q = win_on ? p.lane2 + query : nullptr;
     float pub2 = -INFINITY;   // last second-best published
-    unsigned nx2[kWin];       // the window as read at the end of the previous accumulator
+    unsigned nx2[kWin];       // the window as read at the end of the previous tile
     bool have2 = false;
 
-    long long w_tfull = 0, busy = 0, slow_chunks = 0;
-    int it = 0;
-    for (int ti = tl; ti < walk_tiles; ti += TL, ++it) {
-      if (have2) {  // in the shadow of the wait for the MMA
-        const unsigned kb = window_bound<kKL>(nx2);
-        L.nxt_key = kb > L.nxt_key ? kb : L.nxt_key;
-        have2 = false;
-      }
+    const uint64_t a_desc0 = make_kmajor_sw128_desc(a_smem(0) + g * (64 * kBlockK * 2));
+    const uint64_t b_desc0 = make_kmajor_sw128_desc(b_smem(0));
+    constexpr uint64_t kStageDesc = Cfg::kStageBytes >> 4;  // one stage further in the descriptors' address field
+    int stage = 0;
+    uint32_t phase = 0;
+    long long w_full = 0, w_stage = 0, w_mma = 0, busy = 0, slow_chunks = 0;
+    for (int ti = tl; ti < walk_tiles; ti += TL) {
       const int t = ti * p.tile_stride;
-      const float qnan = __int_as_float(0x7fc00000);
-      auto sc = [&](float x) { return x > 0.f ? x : qnan; };
-      float4* dst = reinterpret_cast<float4*>(ic + 8 * lane);
-      dst[0] = make_float4(sc(nx0.x), sc(nx0.y), sc(nx0.z), sc(nx0.w));
-      dst[1] = make_float4(sc(nx1.x), sc(nx1.y), sc(nx1.z), sc(nx1.w));
-      if (ti + TL < walk_tiles) fetch_ic((ti + TL) * p.tile_stride);  // prefetch the next tile's inverse norms
-      __syncwarp();                                // ic[] visible to the whole warp
-      const int a = it & 1;
-      const uint32_t aph = (it >> 1) & 1u;
-      long long c0 = 0;
-      if constexpr (kProf) c0 = clock64();
-      mbar_wait(tfull_bar(a), aph, static_cast<uint32_t>(p.wait_hint_ns));
-      tc_fence_after();
-      long long c1 = 0;
-      if constexpr (kProf) c1 = clock64();
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(ew * 32) << 16) + static_cast<uint32_t>(a * kBlockN);
+      int slow = 0;
+      if (epi) {
+        if (have2) {
+          const unsigned kb = window_bound<kKL>(nx2);
+          L.nxt_key = kb > L.nxt_key ? kb : L.nxt_key;
+          have2 = false;
+        }
+        L.apply_shared(L.nxt_key);
+        const float qnan = __int_as_float(0x7fc00000);
+        auto sc = [&](float x) { return x > 0.f ? x : qnan; };
+        float4* dst = reinterpret_cast<float4*>(ic + 8 * lane);
+        dst[0] = make_float4(sc(nx0.x), sc(nx0.y), sc(nx0.z), sc(nx0.w));
+        dst[1] = make_float4(sc(nx1.x), sc(nx1.y), sc(nx1.z), sc(nx1.w));
+        if (ti + TL < walk_tiles) fetch_ic((ti + TL) * p.tile_stride);  // prefetch the next tile's inverse norms
+        __syncwarp();                                                     // ic[] visible to the whole warp
+      }
       float* dbg_row = nullptr;
       if constexpr (kMode == kModeDots) {
-        if (p.dbg_dots != nullptr && t == p.dbg_tile) dbg_row = p.dbg_dots + static_cast<size_t>(query) * kBlockN;
+        if (own_query && p.dbg_dots != nullptr && t == p.dbg_tile) dbg_row = p.dbg_dots + static_cast<size_t>(query) * kBlockN;
       }
-      const int slow = epilogue_accumulator<kKL, kMode>(L, taddr, ic, t * kBlockN, dbg_row);
-      tc_fence_before();
-      __syncwarp();  // also orders this tile's ic[] reads before the next tile's writes
-      if (lane == 0) {
-        if constexpr (kCG == 1)
-          mbar_arrive(tempty_bar(a));
-        else
-          mbar_arrive_cluster(tempty_bar(a), 0);  // the MMA issuer lives in the pair's leader CTA
-      }
-      if constexpr (kProf) {
-        w_tfull += c1 - c0;
-        busy += clock64() - c1;
-        slow_chunks += slow;
-      }
-      // accumulator released: publish this lane's second best and, while the lists are young (or whenever a warp just
-      // paid for insertions), fetch the window for the next accumulator's bound
-      if (p.lane2 != nullptr && TL >= kWin) {
-        const bool fetch = (it < kWinWarmTiles) || __any_sync(0xffffffffu, slow > 0);
-        if (win_on) {
-          if (L.sc[1] > pub2) {
-            pub2 = L.sc[1];
-            st_relaxed_gpu_u32(win_q + static_cast<size_t>(tl) * win_stride, float_to_key(pub2));
+      for (int h = 0; h < 2; ++h) {
+        // ---- MMA: acc = Q[64 x D] . C[half tile]^T, K slice by K slice; a slot is released once the MMAs reading it
+        // have retired (wait_group 1 after the next slice's issue keeps one slice in flight)
+        float acc[64];  // dead between halves: the first MMA of a half overwrites it
+        int prev_stage = -1;
+        for (int kb = 0; kb < p.num_kb; ++kb) {
+          if constexpr (kProf) {
+            const long long c0 = clock64();
+            mbar_wait(full_bar(stage), phase, static_cast<uint32_t>(p.wait_hint_ns));
+            w_full += clock64() - c0;
+          } else {
+            mbar_wait(full_bar(stage), phase, static_cast<uint32_t>(p.wait_hint_ns));
           }
-          if (fetch && ti + TL < walk_tiles) {
+          wgmma_fence();
+          wgmma_fence_operands(acc);
 #pragma unroll
-            for (int i = 0; i < kWin; ++i) {
-              int ln = tl + i;
-              ln -= (ln >= TL) ? TL : 0;
-              nx2[i] = ld_relaxed_gpu_u32(win_q + static_cast<size_t>(ln) * win_stride);
+          for (int k = 0; k < kBlockK / kUmmaK; ++k) {
+            // +32 B along K inside the 128-B swizzle atom = +2 in the (addr >> 4) field
+            wgmma_m64n128k16_bf16(acc, a_desc0 + stage * kStageDesc + 2u * k, b_desc0 + stage * kStageDesc + 2u * k,
+                                  (kb | k) != 0 ? 1u : 0u);
+          }
+          wgmma_commit();
+          wgmma_fence_operands(acc);
+          if (prev_stage >= 0) {
+            wgmma_wait<1>();
+            if (signaller) {
+              mbar_arrive(empty_bar(prev_stage));
+              if constexpr (kCG == 2) mbar_arrive_cluster(empty_bar(prev_stage), rank ^ 1u);
             }
-            have2 = true;
+          }
+          prev_stage = stage;
+          if (++stage == kStages) {
+            stage = 0;
+            phase ^= 1u;
+          }
+        }
+        long long c0 = 0;
+        if constexpr (kProf) c0 = clock64();
+        wgmma_wait<0>();
+        wgmma_fence_operands(acc);
+        if (signaller) {
+          mbar_arrive(empty_bar(prev_stage));
+          if constexpr (kCG == 2) mbar_arrive_cluster(empty_bar(prev_stage), rank ^ 1u);
+        }
+        long long c1 = 0;
+        if constexpr (kProf) c1 = clock64();
+        // ---- stage the accumulators: the previous half's readers are done with the buffer first
+        named_bar_sync(named_bar, 128);
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+          const int r = 16 * (wt >> 5) + ((wt & 31) >> 2);
+          const int col = 8 * j + 2 * (wt & 3);
+          *reinterpret_cast<float2*>(stg + r * kStagingLd + col) = make_float2(acc[4 * j + 0], acc[4 * j + 1]);
+          *reinterpret_cast<float2*>(stg + (r + 8) * kStagingLd + col) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+        }
+        named_bar_sync(named_bar, 128);
+        long long c2 = 0;
+        if constexpr (kProf) c2 = clock64();
+        if (epi)
+          slow += epilogue_half<kKL, kMode>(L, stg + wt * kStagingLd, ic + h * kHalfN, t * kBlockN + h * kHalfN,
+                                            dbg_row != nullptr ? dbg_row + h * kHalfN : nullptr);
+        if constexpr (kProf) {
+          w_mma += c1 - c0;
+          w_stage += c2 - c1;
+          busy += clock64() - c2;
+        }
+      }
+      if constexpr (kProf) slow_chunks += slow;
+      if (epi) {
+        if (L.slot != nullptr) {
+          if (L.sc[kKL - 1] > L.published) {  // list full and its tail improved: tell the other lanes
+            L.published = L.sc[kKL - 1];
+            atomicMax(L.slot, float_to_key(L.published));
+          }
+          L.nxt_key = ld_relaxed_gpu_u32(L.slot);  // consumed at the start of the next tile: latency hidden
+        }
+        // publish this lane's second best and, while the lists are young (or whenever a warp just paid for
+        // insertions), fetch the window for the next tile's bound
+        if (p.lane2 != nullptr && TL >= kWin) {
+          const bool fetch = (ti - tl) / TL < kWinWarmTiles || __any_sync(0xffffffffu, slow > 0);
+          if (win_on) {
+            if (L.sc[1] > pub2) {
+              pub2 = L.sc[1];
+              st_relaxed_gpu_u32(win_q + static_cast<size_t>(tl) * win_stride, float_to_key(pub2));
+            }
+            if (fetch && ti + TL < walk_tiles) {
+#pragma unroll
+              for (int i = 0; i < kWin; ++i) {
+                int ln = tl + i;
+                ln -= (ln >= TL) ? TL : 0;
+                nx2[i] = ld_relaxed_gpu_u32(win_q + static_cast<size_t>(ln) * win_stride);
+              }
+              have2 = true;
+            }
           }
         }
       }
     }
 
     // The only global writes of the scan: this CTA's candidate list and drop bound for each of its queries.
-    if (query < p.nq) {
+    if (own_query) {
       const size_t o = (static_cast<size_t>(blockIdx.x) * kBlockM + et) * kKL;
       float4* ps = reinterpret_cast<float4*>(p.part_score + o);
       int4* pi = reinterpret_cast<int4*>(p.part_idx + o);
@@ -648,8 +636,10 @@ sa_scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant
       p.part_drop[static_cast<size_t>(blockIdx.x) * kBlockM + et] = L.drop;
     }
     if constexpr (kProf) {
-      if (ew == 0 && lane == 0) {
-        p.prof[blockIdx.x].epi_wait_tfull = w_tfull;
+      if (g == 0 && signaller) {
+        p.prof[blockIdx.x].mma_wait_full = w_full;
+        p.prof[blockIdx.x].mma_wait_tempty = w_stage;
+        p.prof[blockIdx.x].epi_wait_tfull = w_mma;
         p.prof[blockIdx.x].epi_busy = busy;
         p.prof[blockIdx.x].epi_slow_chunks = slow_chunks;
       }
@@ -657,17 +647,12 @@ sa_scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant
   }
 
   // ------------------------------------------------------------------ teardown
-  tc_fence_before();
   __syncthreads();
   if (p.dbg_times != nullptr && threadIdx.x == 0) p.dbg_times[2 * blockIdx.x + 1] = globaltimer_ns();
   if constexpr (kProf) {
     if (threadIdx.x == 0) p.prof[blockIdx.x].total = clock64() - t_start;
   }
-  if constexpr (kCG == 2) cluster_sync_all();  // the peer may still be signalling our barriers / reading our smem
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc<kCG>(tmem_base, kTmemCols);
-  }
+  if constexpr (kCG == 2) cluster_sync_all();  // the peer may still be multicasting into our smem / arriving on our barriers
 }
 #endif  // __CUDACC__
 

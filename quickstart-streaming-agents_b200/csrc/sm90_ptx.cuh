@@ -1,0 +1,213 @@
+// sm_90a device primitives used by the scan kernel: mbarrier, TMA (cp.async.bulk.tensor, with cluster
+// multicast), wgmma (warpgroup MMA from shared-memory descriptors, fp32 accumulators in registers).
+//
+// Everything here is inline PTX for sm_90a only; there is no fallback path.  The descriptor bit layout
+// follows the PTX ISA "matrix descriptor" table for wgmma (see DESIGN.md section 4).
+#pragma once
+#include <cstdint>
+#include <cuda.h>
+
+namespace sa {
+
+#ifndef SA_WATCHDOG_CYCLES
+// A barrier wait that lasts this many SM cycles (~2 s) is a protocol bug: trap instead of hanging the box.
+#define SA_WATCHDOG_CYCLES (4000000000ll)
+#endif
+
+__device__ __forceinline__ uint32_t smem_u32(const void* p) {
+  return static_cast<uint32_t>(__cvta_generic_to_shared(p));
+}
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+
+// ----------------------------------------------------------------------------------------------
+// mbarrier
+// ----------------------------------------------------------------------------------------------
+__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
+  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
+}
+__device__ __forceinline__ void fence_mbar_init() {
+  asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+}
+__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
+  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
+}
+// Arrive on the barrier at the same smem offset in CTA `cta` of this cluster.
+__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar, uint32_t cta) {
+  asm volatile(
+      "{\n\t.reg .b32 r;\n\t"
+      "mapa.shared::cluster.u32 r, %0, %1;\n\t"
+      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [r];\n\t}" ::"r"(bar),
+      "r"(cta)
+      : "memory");
+}
+__device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
+  uint32_t ok;
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
+      "selp.u32 %0, 1, 0, p;\n\t}"
+      : "=r"(ok)
+      : "r"(bar), "r"(parity)
+      : "memory");
+  return ok != 0;
+}
+// try_wait with a suspend-time hint: the thread may sleep in hardware for up to `hint_ns` (or until the phase completes)
+// instead of returning to poll -- fewer issue slots and less power for warps that wait most of the time.
+__device__ __forceinline__ bool mbar_try_wait_hint(uint32_t bar, uint32_t parity, uint32_t hint_ns) {
+  uint32_t ok;
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2, %3;\n\t"
+      "selp.u32 %0, 1, 0, p;\n\t}"
+      : "=r"(ok)
+      : "r"(bar), "r"(parity), "r"(hint_ns)
+      : "memory");
+  return ok != 0;
+}
+__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity, uint32_t hint_ns = 0) {
+  if (mbar_try_wait(bar, parity)) return;
+  const long long t0 = clock64();
+  while (!(hint_ns ? mbar_try_wait_hint(bar, parity, hint_ns) : mbar_try_wait(bar, parity))) {
+    // no printf here: a call inside the wgmma loop would make ptxas serialise the warpgroup MMAs
+    if (clock64() - t0 > SA_WATCHDOG_CYCLES) __trap();
+  }
+}
+
+// Named barrier over `nthreads` threads (whole warps) of this CTA; id 0 is __syncthreads'.
+__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
+
+// ----------------------------------------------------------------------------------------------
+// gpu-scope flags in global memory
+// ----------------------------------------------------------------------------------------------
+__device__ __forceinline__ long long globaltimer_ns() {
+  long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
+__device__ __forceinline__ int ld_relaxed_gpu(const int* p) {
+  int v;
+  asm volatile("ld.relaxed.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+  return v;
+}
+__device__ __forceinline__ unsigned ld_relaxed_gpu_u32(const unsigned* p) {
+  unsigned v;
+  asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+  return v;
+}
+__device__ __forceinline__ void st_relaxed_gpu(int* p, int v) {
+  asm volatile("st.relaxed.gpu.global.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+__device__ __forceinline__ void st_relaxed_gpu_u32(unsigned* p, unsigned v) {
+  asm volatile("st.relaxed.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+
+// ----------------------------------------------------------------------------------------------
+// Cluster
+// ----------------------------------------------------------------------------------------------
+__device__ __forceinline__ void cluster_sync_all() {
+  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
+  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+
+// ----------------------------------------------------------------------------------------------
+// TMA
+// ----------------------------------------------------------------------------------------------
+// L2 cache-policy words accepted by the .L2::cache_hint operand (createpolicy encodings).
+constexpr uint64_t kEvictNormal = 0x1000000000000000ull;
+constexpr uint64_t kEvictFirst = 0x12F0000000000000ull;
+constexpr uint64_t kEvictLast = 0x14F0000000000000ull;
+
+__device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* m) {
+  asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(m)) : "memory");
+}
+// 2-D tiled load global -> this CTA's smem, completion bytes on this CTA's mbarrier.
+__device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* m, uint32_t bar, int x, int y,
+                                            uint64_t hint) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
+      " [%0], [%1, {%3, %4}], [%2], %5;" ::"r"(dst),
+      "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(x), "r"(y), "l"(hint)
+      : "memory");
+}
+// Same box, written to the same smem offset in every CTA of `cta_mask`; each destination CTA's mbarrier at offset
+// `bar` is credited with the bytes that landed in that CTA.
+__device__ __forceinline__ void tma_load_2d_multicast(uint32_t dst, const CUtensorMap* m, uint32_t bar, int x, int y,
+                                                      uint16_t cta_mask, uint64_t hint) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster.L2::cache_hint"
+      " [%0], [%1, {%3, %4}], [%2], %5, %6;" ::"r"(dst),
+      "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(x), "r"(y), "h"(cta_mask), "l"(hint)
+      : "memory");
+}
+
+// ----------------------------------------------------------------------------------------------
+// wgmma
+// ----------------------------------------------------------------------------------------------
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+// Wait until at most N of this warpgroup's committed wgmma groups are pending.
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+}
+
+constexpr int kWgmmaN = 128;  // columns (corpus rows) of one warpgroup MMA; 64 fp32 accumulators per thread
+
+// D[64 x 128] (+)= A[64 x 16] * B[128 x 16]^T from shared memory; bf16 inputs, fp32 accumulate, both K-major.
+// Thread t of the warpgroup holds, for j = 0 .. 15, rows 16 (t/32) + (t%32)/4 (+8 for d[4j+2], d[4j+3]) and columns
+// 8j + 2 (t%4) (+1) of D in d[4j .. 4j+3].
+__device__ __forceinline__ void wgmma_m64n128k16_bf16(float (&d)[64], uint64_t a_desc, uint64_t b_desc,
+                                                      uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(a_desc), "l"(b_desc), "r"(accumulate)
+      : "memory");
+}
+// Keeps the compiler from moving reads or writes of the accumulators across a wgmma fence / wait.
+__device__ __forceinline__ void wgmma_fence_operands(float (&d)[64]) {
+#pragma unroll
+  for (int i = 0; i < 64; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// ----------------------------------------------------------------------------------------------
+// Descriptors
+// ----------------------------------------------------------------------------------------------
+// Shared-memory matrix descriptor for a K-major operand tile stored as TMA SWIZZLE_128B rows of 64 bf16
+// (128 B): rows are 128 B apart, 8-row groups 1024 B apart, tile base 1024-B aligned (base offset 0).
+//   [0,14)  start address >> 4      [16,30) leading-dim byte offset >> 4 (unused for swizzled K-major, =1)
+//   [32,46) stride-dim byte offset >> 4 (1024 B between 8-row groups = 64)
+//   [49,52) base offset (0)          [62,64) layout type (1 = SWIZZLE_128B)
+__device__ __forceinline__ uint64_t make_kmajor_sw128_desc(uint32_t smem_addr) {
+  uint64_t d = 0;
+  d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
+  d |= static_cast<uint64_t>(1) << 16;
+  d |= static_cast<uint64_t>(1024 >> 4) << 32;
+  d |= static_cast<uint64_t>(1) << 62;
+  return d;
+}
+
+}  // namespace sa

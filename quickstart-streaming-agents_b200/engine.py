@@ -1,4 +1,4 @@
-"""VectorIndex -- the host-side handle of one corpus shard on one B200.
+"""VectorIndex -- the host-side handle of one corpus shard on one H100.
 
 Plays the role of the reference's external vector table ``documents_vectordb_lab2`` (connector 'mongodb',
 index 'vector_index', cosine, 1536-d: terraform/lab2-vector-search/main.tf:215,
@@ -51,7 +51,7 @@ class VectorIndex:
     def __init__(self, dim: int = 1536, capacity: int = 1 << 20, max_batch: int = 1024, max_k: int = 10,
                  device: int | None = None):
         if not torch.cuda.is_available():
-            raise RuntimeError("VectorIndex needs a CUDA device (B200, sm_100a); there is no CPU fallback")
+            raise RuntimeError("VectorIndex needs a CUDA device (H100, sm_90a); there is no CPU fallback")
         self.lib = capi.load()
         self.device = torch.cuda.current_device() if device is None else int(device)
         self.dim, self.capacity, self.max_batch, self.max_k = int(dim), int(capacity), int(max_batch), int(max_k)

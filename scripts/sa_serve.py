@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""sa_serve -- run the Lab2 topic graph locally on the B200s of this box.
+"""sa_serve -- run the Lab2 topic graph locally on the GPUs of this box.
 
 Consumes ``documents`` / ``queries`` (and pre-embedded ``documents_embed`` / ``queries_embed``) from the topic log,
 keeps the vector table in HBM, writes ``search_results`` and ``search_results_response``

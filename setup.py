@@ -1,5 +1,5 @@
 """pip install .  -- packages the hyphenated source directory as the importable package ``qsa_b200`` together with the
-C ABI: libsa_b200.so (built here with nvcc for sm_100a if it is not there yet) and the headers (qsa_b200/include/*.h).
+C ABI: libsa_b200.so (built here with nvcc for sm_90a if it is not there yet) and the headers (qsa_b200/include/*.h).
 A source checkout needs none of this: ``qsa_b200/__init__.py`` there is a path shim onto the same directory."""
 import os
 import shutil

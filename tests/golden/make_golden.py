@@ -1,8 +1,8 @@
 """Regenerates tests/golden/cosine_topk_*.npz: small seeded inputs and the float64 oracle's answers.
 
 The reference holds no golden vector for this arithmetic (SURVEY.md section 8c: parity unpinned), so these
-fixtures pin the ORACLE's behaviour over time (and travel to the GPU box, where /root/reference does not
-exist).  Run from the repo root:  python tests/golden/make_golden.py
+fixtures pin the ORACLE's behaviour over time (and keep the tests independent of a reference checkout).
+Run from the repo root:  python tests/golden/make_golden.py
 """
 import os
 import sys

@@ -23,8 +23,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 
 CASES = {
     # name: (n, dim, nq, k, seed)
-    "d256_n3000_q40_k10": (3000, 256, 40, 10, 7001),
-    "d1536_n600_q12_k5": (600, 1536, 12, 5, 7002),
+    "d256_n2000_q40_k10": (2000, 256, 40, 10, 7001),       # sizes keep every file under 1 MB
+    "d1536_n360_q12_k5": (360, 1536, 12, 5, 7002),
 }
 
 

@@ -77,8 +77,8 @@ def test_preheat_single_rank_stops_on_stable_or_timeout():
 
 
 def test_step_size_estimate_ignores_one_time_costs():
-    """The batches-per-step estimate must come from settled batches: a slow first call (NCCL connection set-up took 0.3 s
-    once and produced a 0.06 s 'timed region' at N = 8) may not leak into it."""
+    """The seconds-per-batch estimate must come from settled batches: a slow first call (NCCL connection set-up took
+    0.3 s once) may not leak into it."""
     sys.path.insert(0, ROOT)
     import bench
 
@@ -90,9 +90,9 @@ def test_step_size_estimate_ignores_one_time_costs():
     def step():
         calls[0] += 1
         time.sleep(0.25 if calls[0] == 1 else 0.002)
-    inner, ph_s, n_ph, est = bench.settle_and_estimate(step, lambda: None, lambda: None, Sampler(), 1, None, steps=10,
-                                                       min_timed_s=0.5, preheat_max=0.4, settle_s=0.1)
-    assert est < 0.01 and 15 <= inner <= 30            # ~2.2 ms per batch -> ~23 batches per step, not 1
+    ph_s, n_ph, est = bench.settle_and_estimate(step, lambda: None, lambda: None, Sampler(), 1, None, preheat_max=0.4,
+                                                settle_s=0.1)
+    assert 0.002 <= est < 0.01                         # ~2.2 ms per batch, not the 0.25 s first call
     assert n_ph >= 4 and ph_s < 0.5
 
 
@@ -142,7 +142,7 @@ def test_reference_arm_prints_the_contract_line():
 
 
 def test_harness_and_tool_scripts_compile():
-    """The GPU harness can only run on a B200 box; at least keep it syntactically alive here."""
+    """The GPU harness can only run on an H100; at least keep it syntactically alive here."""
     import glob
     import py_compile
     files = glob.glob(os.path.join(ROOT, "tools", "*.py")) + glob.glob(os.path.join(ROOT, "tests", "harness", "*.py")) + \

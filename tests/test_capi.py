@@ -1,8 +1,9 @@
-"""CPU tests of the boundary: libsa_b200.so builds for sm_100a without a GPU, loads, exports every symbol
+"""CPU tests of the boundary: libsa_b200.so builds for sm_90a without a GPU, loads, exports every symbol
 include/sa_api.h declares, and fails loudly (no fallback) when there is no CUDA device."""
 import ctypes as C
 import os
 import re
+import shutil
 import subprocess
 
 import pytest
@@ -11,6 +12,7 @@ import torch
 from qsa_b200 import capi
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+CUOBJDUMP = shutil.which("cuobjdump") or os.path.join(os.environ.get("CUDA_HOME", "/usr/local/cuda"), "bin", "cuobjdump")
 
 
 def header_functions():
@@ -33,14 +35,14 @@ def test_library_exports_every_symbol(lib):
     assert lib.sa_strerror(capi.SA_ERR_DEVICE).decode().startswith("unsupported device")
 
 
-def test_library_contains_only_sm100a_native_code(lib):
-    out = subprocess.run(["cuobjdump", "-lelf", capi.LIB_PATH], capture_output=True, text=True).stdout
-    assert "sm_100a" in out
-    assert not re.search(r"sm_(?!100a)\d+", out), out
-    sass = subprocess.run(["cuobjdump", "-sass", capi.LIB_PATH], capture_output=True, text=True).stdout
-    for mnemonic in ("UTCHMMA", "UTMALDG", "LDTM", "UTCBAR"):   # tcgen05.mma, TMA, tcgen05.ld, tcgen05.commit
+def test_library_contains_only_sm90a_native_code(lib):
+    out = subprocess.run([CUOBJDUMP, "-lelf", capi.LIB_PATH], capture_output=True, text=True).stdout
+    assert "sm_90a" in out
+    assert not re.search(r"sm_(?!90a)\d+", out), out
+    sass = subprocess.run([CUOBJDUMP, "-sass", capi.LIB_PATH], capture_output=True, text=True).stdout
+    for mnemonic in ("HGMMA.64x128x16.F32.BF16", "UTMALDG.2D", "UTMALDG.2D.MULTICAST"):   # wgmma, TMA, TMA multicast
         assert mnemonic in sass, mnemonic
-    assert "HMMA." not in sass.replace("UTCHMMA", "")          # no legacy mma.sync path
+    assert "HMMA." not in sass                                  # no legacy mma.sync path
 
 
 def test_argument_validation_without_touching_the_gpu(lib):
@@ -84,7 +86,7 @@ def plan(lib, num_sms, nq, cg, num_tiles, cap=0):
 @pytest.mark.parametrize("sms", [148, 160])
 def test_launch_planner_invariants(lib, cg, nq, num_tiles, sms):
     """Host logic of the scan: every query is covered exactly once, a launch never needs more CTAs than SMs,
-    tile lanes never outnumber tiles nor the merge kernel's 148-lane table, and the machine is used when the batch
+    tile lanes never outnumber tiles nor the merge kernel's 132-lane table, and the machine is used when the batch
     allows it."""
     launches = plan(lib, sms, nq, cg, num_tiles)
     rows = 128 * cg
@@ -92,7 +94,7 @@ def test_launch_planner_invariants(lib, cg, nq, num_tiles, sms):
     for q0, n, nqb, tl in launches:
         assert q0 == nxt and n > 0 and q0 % rows == 0
         assert nqb == (n + rows - 1) // rows and tl >= 1
-        assert nqb * tl * cg <= sms and tl <= max(num_tiles, 1) and tl <= 148
+        assert nqb * tl * cg <= sms and tl <= max(num_tiles, 1) and tl <= 132
         nxt += n
     assert nxt == nq
     if num_tiles >= 148 and nq >= rows:
@@ -101,9 +103,10 @@ def test_launch_planner_invariants(lib, cg, nq, num_tiles, sms):
 
 
 def test_launch_planner_headline_shapes(lib):
-    assert plan(lib, 148, 1024, 2, 39063) == [(0, 1024, 4, 18)]             # 4 pair blocks x 18 lanes = 72 pairs
-    assert plan(lib, 148, 128, 1, 39063) == [(0, 128, 1, 148)]              # HBM-bound: every SM its own lane
-    assert plan(lib, 148, 512, 2, 39063) == [(0, 512, 2, 37)]               # already fills the machine
-    p = plan(lib, 148, 4096, 2, 4883)                                       # config 4 per GPU: 2 launches of 8 x 9
-    assert [x[2:] for x in p] == [(8, 9), (8, 9)]
-    assert len(plan(lib, 148, 1100, 2, 118, cap=2)) == 3                    # forced small launches
+    assert plan(lib, 132, 1024, 2, 39063) == [(0, 512, 2, 33), (512, 512, 2, 33)]   # 2 launches of 2 pair blocks x 33 lanes
+    assert plan(lib, 132, 128, 1, 39063) == [(0, 128, 1, 132)]              # HBM-bound: every SM its own lane
+    assert plan(lib, 148, 128, 1, 39063) == [(0, 128, 1, 132)]              # ... capped at the merge kernel's 132 lanes
+    assert plan(lib, 132, 512, 2, 39063) == [(0, 512, 2, 33)]               # already fills the machine
+    p = plan(lib, 132, 4096, 2, 4883)                                       # config 4 per GPU: 6 launches
+    assert [x[2:] for x in p] == [(3, 22)] * 4 + [(2, 33)] * 2
+    assert len(plan(lib, 132, 1100, 2, 118, cap=2)) == 3                    # forced small launches
