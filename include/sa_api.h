@@ -33,8 +33,19 @@ typedef enum sa_status {
   SA_ERR_ARG = -2,      /* bad argument (null, range, alignment, dim % 64 != 0, k > max_k ...) */
   SA_ERR_COMM = -3,     /* NCCL could not be loaded / a collective call failed (sa_comm_*) */
   SA_ERR_CAPACITY = -4, /* append past capacity_rows, batch past max_batch */
-  SA_ERR_DEVICE = -5    /* device is not compute capability 10.x */
+  SA_ERR_DEVICE = -5    /* device is not compute capability 9.0 */
 } sa_status;
+
+/* Similarity of an index, fixed at creation (Atlas's vector index "similarity": cosine, dotProduct, euclidean).
+ * The ranking and the returned score per similarity (all arithmetic over the bf16-rounded values, sums in float64):
+ *   SA_SIM_COSINE     cosine desc, row asc;         score = cosine;        all-zero rows are never returned
+ *   SA_SIM_DOT        <q,c> desc, row asc;          score = <q,c>;         an all-zero row is a live row (score 0)
+ *   SA_SIM_EUCLIDEAN  |q - c| asc, row asc;         score = |q - c| = sqrt(max(0, (|q|^2 - 2<q,c>) + |c|^2));
+ *                                                   an all-zero row is a live row (distance |q|)
+ * Empty result slots hold row -1 with the worst value: -inf, or +inf for distances. */
+#define SA_SIM_COSINE 0
+#define SA_SIM_DOT 1
+#define SA_SIM_EUCLIDEAN 2
 
 #define SA_MAX_K 28 /* candidate lists hold 16 (k <= 16) or 32 entries per tile lane */
 #define SA_HOST_SLOTS 2 /* host-buffer searches that may be in flight at once (sa_search_host_submit) */
@@ -49,34 +60,46 @@ const char* sa_last_error(void); /* thread-local detail of the last failure on t
  *   'mongodb.index'='vector_index', 'mongodb.embedding_column'='embedding', ...)
  *   (terraform/lab2-vector-search/main.tf:215) and the index definition {numDimensions 1536, similarity cosine}
  *   (assets/pre-setup/MongoDB-Setup.md:72-83, scripts/common/validate.py:56-61,167-180).
- * dim must be a multiple of 64 (1536 and 768 are); capacity_rows < 2^31; max_k <= SA_MAX_K. */
+ * dim must be a multiple of 64 (1536 and 768 are); capacity_rows < 2^31; max_k <= SA_MAX_K.  sa_engine_create makes a
+ * cosine index; sa_engine_create_sim takes the similarity (SA_SIM_*) and rejects any other value with SA_ERR_ARG before
+ * it touches a device. */
 int sa_engine_create(sa_engine** out, int device, int dim, int64_t capacity_rows, int max_batch, int max_k);
+int sa_engine_create_sim(sa_engine** out, int device, int dim, int64_t capacity_rows, int max_batch, int max_k,
+                         int similarity);
 void sa_engine_destroy(sa_engine* e);
 
 /* Attach caller-owned device storage: rows_bf16 is [capacity_rows x dim] row-major bf16 (16-byte aligned),
- * inv_norm is [capacity_rows] fp32.  n_valid rows are taken as already committed (their inv_norm valid). */
-int sa_corpus_bind(sa_engine* e, void* rows_bf16_dev, float* inv_norm_dev, int64_t n_valid);
+ * row_term is [capacity_rows] fp32 (16-byte aligned), one term per row that the scan combines with <q,c>:
+ *   cosine      1/|c| over the bf16 values, 0 for an all-zero row or a tombstone
+ *   dotProduct  1 for a live row, 0 for a tombstone
+ *   euclidean   |c|^2/2 (summed in fp64, rounded once to fp32) for a live row, negative (e.g. -1) for a tombstone
+ * The ingest entry points below write it; a caller that tombstones a row writes the row's term itself (and may zero the
+ * row).  n_valid rows are taken as already committed (their terms valid); for dotProduct and euclidean the bound on the
+ * rows' norms that the search's certificate uses is recomputed over them. */
+int sa_corpus_bind(sa_engine* e, void* rows_bf16_dev, float* row_term_dev, int64_t n_valid);
 
 /* --- ingest (the "documents -> documents_embed -> MongoDB sink" half of Lab2, LAB2-Walkthrough.md:41-51,
  *     fed by scripts/publish_docs.py:225-351; embeddings arrive as ARRAY<FLOAT>, main.tf:141,215) ------- */
-/* Rows [first_row, first_row+n_new) were written in place as bf16 by the caller: compute their inverse
- * L2 norms and publish them (first_row must equal the current row count). */
+/* Rows [first_row, first_row+n_new) were written in place as bf16 by the caller: compute their row terms and
+ * publish them (first_row must equal the current row count). */
 int sa_corpus_commit(sa_engine* e, int64_t first_row, int64_t n_new, uintptr_t stream);
-/* Convert n_new fp32 rows (device) to bf16 (round-to-nearest-even), append, norm, publish. */
+/* Convert n_new fp32 rows (device) to bf16 (round-to-nearest-even), append, compute row terms, publish. */
 int sa_corpus_append_f32(sa_engine* e, const float* rows_f32_dev, int64_t n_new, uintptr_t stream);
 /* Same from host memory (staged through pinned memory in chunks); blocking. */
 int sa_corpus_append_host_f32(sa_engine* e, const float* rows_f32_host, int64_t n_new);
-/* Forget all rows -- what scripts/common/clear_mongodb.py:98-158 (delete_many({})) does to the collection. */
+/* Forget all rows -- what scripts/common/clear_mongodb.py:98-158 (delete_many({})) does to the collection.  For
+ * dotProduct and euclidean it also clears the norm bound, and then waits for the device. */
 int sa_corpus_reset(sa_engine* e);
 int64_t sa_corpus_rows(const sa_engine* e);
 
 /* --- search: LATERAL TABLE(VECTOR_SEARCH_AGG(documents_vectordb_lab2, DESCRIPTOR(embedding),
  *     qe.embedding, k))  (terraform/lab2-vector-search/main.tf:292; LAB3-Walkthrough.md:343-350;
  *     LAB4-Walkthrough.md:302-309) for a batch of nq query vectors --------------------------------------
- * Result for query i: out_idx[i*k .. i*k+k) = shard-local rows of the k most cosine-similar committed corpus
- * rows, descending by cosine, ties by ascending row; out_score = those cosines (fp32 rounding of the fp64
- * value); slots past the number of eligible rows hold idx -1 / score -inf.  All-zero corpus rows are never
- * returned.  out_score64 (optional, may be NULL) receives the unrounded cosines for a cross-shard merge. */
+ * Result for query i: out_idx[i*k .. i*k+k) = shard-local rows of the k best committed corpus rows under the
+ * engine's similarity (see SA_SIM_*: descending cosine or dot product, ascending distance; ties by ascending row);
+ * out_score = their scores (fp32 rounding of the fp64 value); slots past the number of eligible rows hold idx -1 /
+ * score -inf (+inf for distances).  Tombstoned rows are never returned, nor all-zero rows under cosine.
+ * out_score64 (optional, may be NULL) receives the unrounded scores for a cross-shard merge. */
 int sa_search(sa_engine* e, const void* q_bf16_dev, int nq, int k, float* out_score_dev, int32_t* out_idx_dev,
               double* out_score64_dev, uintptr_t stream);
 /* Queries as fp32 (the ML_PREDICT output type, terraform/core/main.tf:500,534): rounded to bf16 first. */
@@ -98,14 +121,15 @@ int sa_search_host_wait(sa_engine* e, int slot, float* out_score_host, int32_t* 
  *     per rank -- and every rank merges them to the global top-k by (cosine desc, global row asc).  This is the whole of
  *     what the sharded VECTOR_SEARCH_AGG (main.tf:292) needs; there is no all-reduce and no all-to-all. ------------------ */
 typedef struct sa_hit {
-  double score; /* cosine, float64 */
+  double score; /* the returned score, float64: cosine, dot product or Euclidean distance (the engine's similarity) */
   int64_t row;  /* global row = shard-local row + row_offset, -1 = no row */
 } sa_hit;
 
 /* This shard's results in exchange format (device buffer [nq x k]), e.g. for a caller-run collective. */
 int sa_search_hits(sa_engine* e, const void* q_bf16_dev, int nq, int k, int64_t row_offset, sa_hit* out_hits_dev,
                    uintptr_t stream);
-/* Merge gathered hit lists [n_shards x nq x k] into the global top-k: out_score [nq x k] fp32, out_row [nq x k] int64. */
+/* Merge gathered hit lists [n_shards x nq x k] into the global top-k: out_score [nq x k] fp32, out_row [nq x k] int64.
+ * The order is that of e's similarity (ascending for distances). */
 int sa_merge_hits(sa_engine* e, const sa_hit* hits_dev, int n_shards, int nq, int k, float* out_score_dev,
                   int64_t* out_row_dev, uintptr_t stream);
 /* Older split form of the same merge (separate score / row arrays). */
@@ -127,6 +151,8 @@ void sa_comm_destroy(sa_comm* c);
 int sa_comm_ranks(const sa_comm* c);
 
 /* One process per GPU: this rank's part of a sharded search (collective: every rank must call it with the same nq, k).
+ * The first search on a communicator also compares the ranks' similarities (one small all-gather, blocking) and every
+ * rank fails with SA_ERR_ARG if they differ; sa_gather_merge* fails the same way if the engines' similarities differ.
  * Device form, asynchronous on `stream`: out_score [nq x k] fp32, out_row [nq x k] int64 global rows, same on all ranks. */
 int sa_sharded_search(sa_comm* c, sa_engine* e, const void* q_bf16_dev, int nq, int k, int64_t row_offset,
                       float* out_score_dev, int64_t* out_row_dev, uintptr_t stream);
@@ -168,7 +194,8 @@ int sa_timing_mean(sa_engine* e, int n, float* scan_ms_mean, float* total_ms_mea
  * "count_fix" = 0 | 1 (record how many (query, lane) pairs the last search sent to the fallback; costs a host sync). */
 int sa_set_option(sa_engine* e, const char* name, int64_t value);
 /* "num_sms", "dim", "capacity", "n_rows", "max_batch", "max_k", "last_grid", "last_fix_entries" (with "count_fix"),
- * "eps_rel_e12" (the certificate's error bound per unit |q|, times 1e12). */
+ * "eps_rel_e12" (the certificate's relative error bound, times 1e12), "similarity" (SA_SIM_*), "cmax_bits" (fp32 bits of
+ * the device-side upper bound on the committed rows' norms; dotProduct and euclidean only, 0 for cosine; synchronous). */
 int sa_get_info(const sa_engine* e, const char* name, int64_t* value);
 /* Per-CTA profile records of the last scan launch run with "profile" = 1 (synchronises the device): out_host receives
  * n_ctas x 8 int64 {TMA producer wait for a free slot, MMA issuer wait for data, MMA issuer wait for the epilogue,

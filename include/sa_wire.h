@@ -56,8 +56,8 @@ int sa_wire_decode_documents_embed(const uint8_t* buf, const uint64_t* value_off
  * appended with one write.  Record i: query text = text_buf[text_off[i] .. +text_len[i]) (text_len 0xFFFFFFFF = null),
  * results j = 0 .. n_out-1 from score[i*k + j] / row[i*k + j] (row < 0 = no hit -> three nulls).  The non-vector columns
  * of the table come pre-serialised as Avro ["null","string"] values in two arenas: column value of table row r is
- * doc_arena[doc_off[r] .. doc_off[r+1]) and chunk_arena[chunk_off[r] .. chunk_off[r+1]).  score_mode 0 = raw cosine,
- * 1 = Atlas (1 + cos) / 2.  out_rec_off[i] receives the offset of record i inside out (out_rec_off[n] = total bytes).
+ * doc_arena[doc_off[r] .. doc_off[r+1]) and chunk_arena[chunk_off[r] .. chunk_off[r+1]).  score_mode 0 = the raw score,
+ * 1 = Atlas's (1 + s) / 2 (cosine, dotProduct), 2 = Atlas's 1 / (1 + d) (euclidean distance d).  out_rec_off[i] receives the offset of record i inside out (out_rec_off[n] = total bytes).
  * Fails with SA_ERR_CAPACITY (and reports the needed size in *needed) when out_cap is too small. */
 int sa_wire_encode_search_results(int n, int k, int n_out, uint32_t schema_id, const uint8_t* text_buf,
                                   const uint64_t* text_off, const uint32_t* text_len, const float* score,

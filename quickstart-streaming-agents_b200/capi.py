@@ -20,10 +20,21 @@ SA_ERR_DEVICE = -5
 SA_MAX_K = 28
 SA_HOST_SLOTS = 2
 SA_COMM_ID_BYTES = 128
+SA_SIM_COSINE = 0
+SA_SIM_DOT = 1
+SA_SIM_EUCLIDEAN = 2
+# Atlas's names for the index's "similarity" setting -> the engine's constants
+SIMILARITIES = {"cosine": SA_SIM_COSINE, "dotProduct": SA_SIM_DOT, "euclidean": SA_SIM_EUCLIDEAN}
+
+
+def similarity_code(name: str) -> int:
+    if name not in SIMILARITIES:
+        raise ValueError(f"similarity must be one of {sorted(SIMILARITIES)}, not {name!r}")
+    return SIMILARITIES[name]
 
 # every symbol include/sa_api.h declares (tests check the .so exports each of them)
 EXPORTS = (
-    "sa_version", "sa_strerror", "sa_last_error", "sa_engine_create", "sa_engine_destroy", "sa_corpus_bind",
+    "sa_version", "sa_strerror", "sa_last_error", "sa_engine_create", "sa_engine_create_sim", "sa_engine_destroy", "sa_corpus_bind",
     "sa_corpus_commit", "sa_corpus_append_f32", "sa_corpus_append_host_f32", "sa_corpus_reset", "sa_corpus_rows",
     "sa_search", "sa_search_f32", "sa_search_host", "sa_search_host_submit", "sa_search_host_wait",
     "sa_search_hits", "sa_merge_hits", "sa_merge_shards",
@@ -67,6 +78,7 @@ def load() -> C.CDLL:
         "sa_strerror": (C.c_char_p, [i32]),
         "sa_last_error": (C.c_char_p, []),
         "sa_engine_create": (i32, [C.POINTER(vp), i32, i32, i64, i32, i32]),
+        "sa_engine_create_sim": (i32, [C.POINTER(vp), i32, i32, i64, i32, i32, i32]),
         "sa_engine_destroy": (None, [vp]),
         "sa_corpus_bind": (i32, [vp, vp, vp, i64]),
         "sa_corpus_commit": (i32, [vp, i64, i64, vp]),

@@ -113,9 +113,11 @@ struct sa_engine {
   int max_batch = 0;
   int max_k = 0;
   int num_sms = 0;
+  int sim = SA_SIM_COSINE;     // fixed at creation
 
   uint16_t* corpus = nullptr;  // caller-owned
-  float* inv_norm = nullptr;   // caller-owned
+  float* row_term = nullptr;   // caller-owned: 1/|c| (cosine), 1 (dotProduct), |c|^2/2 (euclidean); see sa_aux.cuh
+  unsigned* cmax = nullptr;    // device scalar (float bits): upper bound on |c| over the committed rows (not cosine)
   int64_t n_rows = 0;
   CUtensorMap tmap_c[2];       // [0]: box 128 rows (cta_group 1), [1]: box 64 rows (cta_group 2, multicast)
   bool bound = false;
@@ -124,7 +126,7 @@ struct sa_engine {
   float* part_score = nullptr;  // [num_sms][128][32]
   int* part_idx = nullptr;
   float* part_drop = nullptr;   // [num_sms][128]
-  double* res64 = nullptr;      // [max_batch][max_k] internal result of a search: cosine (float64) ...
+  double* res64 = nullptr;      // [max_batch][max_k] internal result of a search: value (float64, larger is better) ...
   int* residx = nullptr;        // ... and shard-local row
   sa::FixEntry* fix_entries = nullptr;  // [kMaxLaunches * num_sms * 128] work queue of the exact fallback scan
   sa::FixQuery* fix_query = nullptr;    // [max_batch]
@@ -196,13 +198,14 @@ struct sa_engine {
 
 namespace {
 
+// asc = 1: the hits are Euclidean distances (smaller is better)
 int launch_merge_packed(const sa::PackedHit* hits, int n_shards, int nq, int k, float* out_score, long long* out_row,
-                        cudaStream_t st) {
+                        int asc, cudaStream_t st) {
   if (n_shards <= 32 && n_shards * k <= 256 && k <= sa::kMergePackedMaxK)
     sa::sa_merge_packed_kernel<<<(nq + sa::kMergePackedWarps - 1) / sa::kMergePackedWarps, sa::kMergePackedWarps * 32, 0, st>>>(
-        hits, n_shards, nq, k, out_score, out_row);
+        hits, n_shards, nq, k, out_score, out_row, asc);
   else
-    sa::sa_merge_packed_serial_kernel<<<(nq + 127) / 128, 128, 0, st>>>(hits, n_shards, nq, k, out_score, out_row);
+    sa::sa_merge_packed_serial_kernel<<<(nq + 127) / 128, 128, 0, st>>>(hits, n_shards, nq, k, out_score, out_row, asc);
   SA_CUDA(cudaGetLastError());
   return SA_OK;
 }
@@ -268,9 +271,9 @@ std::vector<LaunchPlan> plan_search(int num_sms, int max_launch_qblocks, int nq,
   return out;
 }
 
-template <int kCG, int kKL, int kMode>
+template <int kCG, int kKL, int kMode, int kEpi = sa::kEpiMul>
 int launch_scan(const CUtensorMap& tq, const CUtensorMap& tc, const sa::ScanParams& p, int grid, cudaStream_t st) {
-  auto kern = sa::sa_scan_kernel<kCG, kKL, kMode>;
+  auto kern = sa::sa_scan_kernel<kCG, kKL, kMode, kEpi>;
   // per-device attribute; a few microseconds, so set it on every launch rather than caching per device
   SA_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, sa::ScanCfg<kCG>::kSmemBytes));
   cudaLaunchConfig_t cfg = {};
@@ -289,8 +292,23 @@ int launch_scan(const CUtensorMap& tq, const CUtensorMap& tc, const sa::ScanPara
   return SA_OK;
 }
 
-int launch_scan_dispatch(int cg, int kl, int mode, const CUtensorMap& tq, const CUtensorMap& tc, const sa::ScanParams& p,
-                         int grid, cudaStream_t st) {
+// epi: sa::kEpiMul (cosine, dotProduct) or sa::kEpiSub (euclidean).  The debug dump reads raw accumulators, which do
+// not depend on the epilogue, so it has the multiply form only.
+int launch_scan_dispatch(int cg, int kl, int mode, int epi, const CUtensorMap& tq, const CUtensorMap& tc,
+                         const sa::ScanParams& p, int grid, cudaStream_t st) {
+  if (epi == sa::kEpiSub) {
+    if (mode == sa::kModeProf) {
+      if (cg == 1 && kl == 16) return launch_scan<1, 16, sa::kModeProf, sa::kEpiSub>(tq, tc, p, grid, st);
+      if (cg == 2 && kl == 16) return launch_scan<2, 16, sa::kModeProf, sa::kEpiSub>(tq, tc, p, grid, st);
+      return fail(SA_ERR_ARG, "the profiling build of the scan exists for 16-entry lists only");
+    }
+    if (mode != sa::kModeProd) return fail(SA_ERR_ARG, "no euclidean scan instantiation for mode %d", mode);
+    if (cg == 1 && kl == 16) return launch_scan<1, 16, sa::kModeProd, sa::kEpiSub>(tq, tc, p, grid, st);
+    if (cg == 1 && kl == 32) return launch_scan<1, 32, sa::kModeProd, sa::kEpiSub>(tq, tc, p, grid, st);
+    if (cg == 2 && kl == 16) return launch_scan<2, 16, sa::kModeProd, sa::kEpiSub>(tq, tc, p, grid, st);
+    if (cg == 2 && kl == 32) return launch_scan<2, 32, sa::kModeProd, sa::kEpiSub>(tq, tc, p, grid, st);
+    return fail(SA_ERR_ARG, "no scan instantiation for cta_group %d list %d", cg, kl);
+  }
   if (mode == sa::kModeDots) {
     if (cg == 1) return launch_scan<1, 16, sa::kModeDots>(tq, tc, p, grid, st);
     return launch_scan<2, 16, sa::kModeDots>(tq, tc, p, grid, st);
@@ -365,6 +383,7 @@ int do_search(sa_engine* e, const uint16_t* q_bf16, int nq, int k, float* out_sc
   if (static_cast<int>(plan.size()) > kMaxLaunches)
     return fail(SA_ERR_CAPACITY, "batch needs %zu scan launches (max %d)", plan.size(), kMaxLaunches);
   const int mode = e->opt_profile ? sa::kModeProf : sa::kModeProd;
+  const int epi = e->sim == SA_SIM_EUCLIDEAN ? sa::kEpiSub : sa::kEpiMul;
   const float eps_rel = scan_eps_rel(e->dim);
 
   // The candidate lists, shared thresholds and drift counters are one set of scratch buffers: a search issued on
@@ -389,7 +408,7 @@ int do_search(sa_engine* e, const uint16_t* q_bf16, int nq, int k, float* out_sc
     if (rc) return rc;
 
     sa::ScanParams sp = {};
-    sp.inv_norm = e->inv_norm;
+    sp.row_term = e->row_term;
     sp.n_rows = n_rows;
     sp.nq = lp.nq;
     sp.num_kb = e->dim / sa::kBlockK;
@@ -441,7 +460,7 @@ int do_search(sa_engine* e, const uint16_t* q_bf16, int nq, int k, float* out_sc
       pp.pace_gain = 0;
       pp.lane2 = nullptr;
       pp.prof = e->prof;
-      rc = launch_scan_dispatch(lp.cg, kl, sa::kModeProd, tq, e->tmap_c[lp.cg - 1], pp, grid, st);
+      rc = launch_scan_dispatch(lp.cg, kl, sa::kModeProd, epi, tq, e->tmap_c[lp.cg - 1], pp, grid, st);
       if (rc) return rc;
       sa::MergeParams bp = {};
       bp.part_score = e->part_score;
@@ -464,7 +483,7 @@ int do_search(sa_engine* e, const uint16_t* q_bf16, int nq, int k, float* out_sc
       SA_CUDA(cudaGetLastError());
       tm.kernels += 2;
     }
-    rc = launch_scan_dispatch(lp.cg, kl, mode, tq, e->tmap_c[lp.cg - 1], sp, grid, st);
+    rc = launch_scan_dispatch(lp.cg, kl, mode, epi, tq, e->tmap_c[lp.cg - 1], sp, grid, st);
     if (rc) return rc;
     SA_CUDA(cudaEventRecord(tm.ev_scan[li][1], st));
 
@@ -483,6 +502,8 @@ int do_search(sa_engine* e, const uint16_t* q_bf16, int nq, int k, float* out_sc
     mp.unit_map = e->opt_unit_map;
     mp.q0 = lp.q0;
     mp.eps_rel = eps_rel;
+    mp.sim = e->sim;
+    mp.cmax = e->cmax;
     mp.res64 = e->res64 + static_cast<size_t>(lp.q0) * k;
     mp.residx = e->residx + static_cast<size_t>(lp.q0) * k;
     mp.fix_entries = e->fix_entries;
@@ -510,7 +531,7 @@ int do_search(sa_engine* e, const uint16_t* q_bf16, int nq, int k, float* out_sc
     fp.done_count = e->fix_counters + 1;
     fp.fix_query = e->fix_query;
     fp.corpus = e->corpus;
-    fp.inv_norm = e->inv_norm;
+    fp.row_term = e->row_term;
     fp.queries = q_bf16;
     fp.n_rows = n_rows;
     fp.num_tiles = num_tiles;
@@ -519,7 +540,7 @@ int do_search(sa_engine* e, const uint16_t* q_bf16, int nq, int k, float* out_sc
     fp.k = k;
     const int tiles_per_lane = (std::max(num_tiles, 1) + min_tl - 1) / min_tl;
     fp.chunks_per_entry = (tiles_per_lane + sa::kFixChunkTiles - 1) / sa::kFixChunkTiles;
-    fp.eps_rel = eps_rel;
+    fp.sim = e->sim;
     fp.res64 = e->res64;
     fp.residx = e->residx;
     fp.out_score = out_score;
@@ -601,8 +622,15 @@ const char* sa_strerror(int rc) {
 const char* sa_last_error(void) { return g_err; }
 
 int sa_engine_create(sa_engine** out, int device, int dim, int64_t capacity_rows, int max_batch, int max_k) {
+  return sa_engine_create_sim(out, device, dim, capacity_rows, max_batch, max_k, SA_SIM_COSINE);
+}
+
+int sa_engine_create_sim(sa_engine** out, int device, int dim, int64_t capacity_rows, int max_batch, int max_k,
+                         int similarity) {
   if (!out) return fail(SA_ERR_ARG, "null out");
   *out = nullptr;
+  if (similarity != SA_SIM_COSINE && similarity != SA_SIM_DOT && similarity != SA_SIM_EUCLIDEAN)
+    return fail(SA_ERR_ARG, "similarity %d is not SA_SIM_COSINE (0), SA_SIM_DOT (1) or SA_SIM_EUCLIDEAN (2)", similarity);
   if (dim <= 0 || dim % 64 != 0) return fail(SA_ERR_ARG, "dim %d must be a positive multiple of 64", dim);
   if (capacity_rows <= 0 || capacity_rows >= (1ll << 31) - 512)
     return fail(SA_ERR_ARG, "capacity_rows %lld outside (0, 2^31-512)", (long long)capacity_rows);
@@ -621,6 +649,7 @@ int sa_engine_create(sa_engine** out, int device, int dim, int64_t capacity_rows
 
   sa_engine* e = new sa_engine();
   e->device = device;
+  e->sim = similarity;
   e->dim = dim;
   e->capacity = capacity_rows;
   e->max_batch = max_batch;
@@ -647,6 +676,8 @@ int sa_engine_create(sa_engine** out, int device, int dim, int64_t capacity_rows
   SA_TRY(cudaMalloc(&e->fix_entries, static_cast<size_t>(kMaxLaunches) * e->num_sms * 128 * sizeof(sa::FixEntry)));
   SA_TRY(cudaMalloc(&e->fix_query, static_cast<size_t>(max_batch) * sizeof(sa::FixQuery)));
   SA_TRY(cudaMalloc(&e->fix_counters, 2 * sizeof(int)));
+  SA_TRY(cudaMalloc(&e->cmax, sizeof(unsigned)));
+  SA_TRY(cudaMemset(e->cmax, 0, sizeof(unsigned)));
   SA_TRY(cudaMalloc(&e->prof, static_cast<size_t>(e->num_sms) * sizeof(sa::ScanProf)));
   SA_TRY(cudaMemset(e->prof, 0, static_cast<size_t>(e->num_sms) * sizeof(sa::ScanProf)));
   SA_TRY(cudaMalloc(&e->q_bf16, qelems * 2));
@@ -704,6 +735,7 @@ void sa_engine_destroy(sa_engine* e) {
   cudaFree(e->fix_entries);
   cudaFree(e->fix_query);
   cudaFree(e->fix_counters);
+  cudaFree(e->cmax);
   cudaFree(e->prof);
   cudaFree(e->q_bf16);
   cudaFree(e->q_f32);
@@ -736,10 +768,15 @@ void sa_engine_destroy(sa_engine* e) {
   delete e;
 }
 
-int sa_corpus_bind(sa_engine* e, void* rows_bf16_dev, float* inv_norm_dev, int64_t n_valid) {
-  if (!e || !rows_bf16_dev || !inv_norm_dev) return fail(SA_ERR_ARG, "null argument");
+namespace {
+constexpr int kIngestBlock = 256;  // one warp per row
+unsigned ingest_grid(int64_t n) { return static_cast<unsigned>((n * 32 + kIngestBlock - 1) / kIngestBlock); }
+}  // namespace
+
+int sa_corpus_bind(sa_engine* e, void* rows_bf16_dev, float* row_term_dev, int64_t n_valid) {
+  if (!e || !rows_bf16_dev || !row_term_dev) return fail(SA_ERR_ARG, "null argument");
   if (reinterpret_cast<uintptr_t>(rows_bf16_dev) % 16) return fail(SA_ERR_ARG, "corpus must be 16-byte aligned");
-  if (reinterpret_cast<uintptr_t>(inv_norm_dev) % 16) return fail(SA_ERR_ARG, "inv_norm must be 16-byte aligned");
+  if (reinterpret_cast<uintptr_t>(row_term_dev) % 16) return fail(SA_ERR_ARG, "row_term must be 16-byte aligned");
   if (n_valid < 0 || n_valid > e->capacity) return fail(SA_ERR_CAPACITY, "n_valid outside [0, capacity]");
   SA_ON_DEVICE(e->device);
   int rc = encode_rows_map(&e->tmap_c[0], rows_bf16_dev, static_cast<uint64_t>(e->capacity), e->dim,
@@ -749,9 +786,18 @@ int sa_corpus_bind(sa_engine* e, void* rows_bf16_dev, float* inv_norm_dev, int64
                        sa::ScanCfg<2>::kBRows);
   if (rc) return rc;
   e->corpus = static_cast<uint16_t*>(rows_bf16_dev);
-  e->inv_norm = inv_norm_dev;
+  e->row_term = row_term_dev;
   e->n_rows = n_valid;
   e->bound = true;
+  if (e->sim != SA_SIM_COSINE) {
+    // Cmax over the rows taken as committed (the legacy default stream orders this before later work on blocking streams)
+    SA_CUDA(cudaMemsetAsync(e->cmax, 0, sizeof(unsigned), 0));
+    if (n_valid > 0) {
+      sa::sa_rowterm_kernel<sa::kSimDot><<<ingest_grid(n_valid), kIngestBlock, 0, 0>>>(e->corpus, nullptr, -1, n_valid,
+                                                                                      e->dim, e->cmax);
+      SA_CUDA(cudaGetLastError());
+    }
+  }
   return SA_OK;
 }
 
@@ -762,11 +808,15 @@ int sa_corpus_commit(sa_engine* e, int64_t first_row, int64_t n_new, uintptr_t s
   if (n_new < 0 || first_row + n_new > e->capacity) return fail(SA_ERR_CAPACITY, "commit past capacity");
   if (n_new == 0) return SA_OK;
   SA_ON_DEVICE(e->device);
-  const long long threads = n_new * 32;
-  const int block = 256;
-  const long long grid = (threads + block - 1) / block;
-  sa::sa_rownorm_kernel<<<static_cast<unsigned>(grid), block, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      e->corpus, e->inv_norm, first_row, n_new, e->dim);
+  const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (e->sim == SA_SIM_COSINE)
+    sa::sa_rownorm_kernel<<<ingest_grid(n_new), kIngestBlock, 0, st>>>(e->corpus, e->row_term, first_row, n_new, e->dim);
+  else if (e->sim == SA_SIM_DOT)
+    sa::sa_rowterm_kernel<sa::kSimDot><<<ingest_grid(n_new), kIngestBlock, 0, st>>>(e->corpus, e->row_term, first_row,
+                                                                                   n_new, e->dim, e->cmax);
+  else
+    sa::sa_rowterm_kernel<sa::kSimEuc><<<ingest_grid(n_new), kIngestBlock, 0, st>>>(e->corpus, e->row_term, first_row,
+                                                                                   n_new, e->dim, e->cmax);
   SA_CUDA(cudaGetLastError());
   e->n_rows = first_row + n_new;
   return SA_OK;
@@ -779,11 +829,17 @@ int sa_corpus_append_f32(sa_engine* e, const float* rows_f32_dev, int64_t n_new,
   if (n_new < 0 || e->n_rows + n_new > e->capacity) return fail(SA_ERR_CAPACITY, "append past capacity");
   if (n_new == 0) return SA_OK;
   SA_ON_DEVICE(e->device);
-  const long long threads = n_new * 32;
-  const int block = 256;
-  const long long grid = (threads + block - 1) / block;
-  sa::sa_convert_rows_kernel<<<static_cast<unsigned>(grid), block, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      rows_f32_dev, e->corpus + e->n_rows * e->dim, e->inv_norm + e->n_rows, n_new, e->dim);
+  const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  uint16_t* dst = e->corpus + e->n_rows * e->dim;
+  float* w = e->row_term + e->n_rows;
+  if (e->sim == SA_SIM_COSINE)
+    sa::sa_convert_rows_kernel<<<ingest_grid(n_new), kIngestBlock, 0, st>>>(rows_f32_dev, dst, w, n_new, e->dim);
+  else if (e->sim == SA_SIM_DOT)
+    sa::sa_convert_rows_term_kernel<sa::kSimDot><<<ingest_grid(n_new), kIngestBlock, 0, st>>>(rows_f32_dev, dst, w, n_new,
+                                                                                            e->dim, e->cmax);
+  else
+    sa::sa_convert_rows_term_kernel<sa::kSimEuc><<<ingest_grid(n_new), kIngestBlock, 0, st>>>(rows_f32_dev, dst, w, n_new,
+                                                                                            e->dim, e->cmax);
   SA_CUDA(cudaGetLastError());
   e->n_rows += n_new;
   return SA_OK;
@@ -811,6 +867,13 @@ int sa_corpus_append_host_f32(sa_engine* e, const float* rows_f32_host, int64_t 
 
 int sa_corpus_reset(sa_engine* e) {
   if (!e) return fail(SA_ERR_ARG, "null engine");
+  if (e->sim != SA_SIM_COSINE) {
+    // Cmax starts over.  Blocking: an append issued after the reset, on any stream, must raise it after it was cleared.
+    SA_ON_DEVICE(e->device);
+    SA_CUDA(cudaDeviceSynchronize());
+    SA_CUDA(cudaMemset(e->cmax, 0, sizeof(unsigned)));
+    SA_CUDA(cudaDeviceSynchronize());
+  }
   e->n_rows = 0;
   return SA_OK;
 }
@@ -920,6 +983,7 @@ struct sa_comm {
   std::vector<ncclComm_t> comms;    // one per local rank
   std::vector<sa::PackedHit*> gathered;  // per local rank: [n_ranks][cap_nq][cap_k], grown on demand
   std::vector<size_t> gathered_elems;
+  int sim = -1;                     // one process per GPU: the similarity every rank's engine was found to have
 };
 
 namespace {
@@ -961,7 +1025,7 @@ int sharded_search_on_stream(sa_comm* c, int local, sa_engine* e, const uint16_t
     SA_NCCL(g_nccl.AllGather(e->hits, gathered, bytes, ncclChar, c->comms[local], st));
   }
   if (phases & 4) {
-    rc = launch_merge_packed(gathered, c->n_ranks, nq, k, out_score_dev, out_row_dev, st);
+    rc = launch_merge_packed(gathered, c->n_ranks, nq, k, out_score_dev, out_row_dev, e->sim == SA_SIM_EUCLIDEAN, st);
     if (rc) return rc;
     e->ring[(e->n_searches - 1) % kTimingRing].kernels += 2;  // the collective and the shard merge
   }
@@ -1075,7 +1139,7 @@ int sa_merge_shards(sa_engine* e, const double* score64_dev, const int64_t* glob
   SA_ON_DEVICE(e->device);
   sa::sa_merge_shards_kernel<<<(nq + 127) / 128, 128, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       score64_dev, reinterpret_cast<const long long*>(global_idx_dev), n_shards, nq, k, out_score_dev,
-      reinterpret_cast<long long*>(out_idx_dev));
+      reinterpret_cast<long long*>(out_idx_dev), e->sim == SA_SIM_EUCLIDEAN);
   SA_CUDA(cudaGetLastError());
   return SA_OK;
 }
@@ -1101,7 +1165,8 @@ int sa_merge_hits(sa_engine* e, const sa_hit* hits_dev, int n_shards, int nq, in
   if (nq <= 0 || k <= 0) return fail(SA_ERR_ARG, "nq and k must be positive");
   SA_ON_DEVICE(e->device);
   return launch_merge_packed(reinterpret_cast<const sa::PackedHit*>(hits_dev), n_shards, nq, k, out_score_dev,
-                             reinterpret_cast<long long*>(out_row_dev), reinterpret_cast<cudaStream_t>(stream));
+                             reinterpret_cast<long long*>(out_row_dev), e->sim == SA_SIM_EUCLIDEAN,
+                             reinterpret_cast<cudaStream_t>(stream));
 }
 
 // ---- communicator ---------------------------------------------------------------------------------------------------
@@ -1190,10 +1255,31 @@ void sa_comm_destroy(sa_comm* c) {
 int sa_comm_ranks(const sa_comm* c) { return c ? c->n_ranks : -1; }
 
 namespace {
-int check_rank_comm(const sa_comm* c, const sa_engine* e) {
+int check_rank_comm(sa_comm* c, const sa_engine* e) {
   if (!c) return fail(SA_ERR_ARG, "null communicator");
   if (c->rank < 0) return fail(SA_ERR_ARG, "single-process communicator: use sa_gather_merge");
   if (c->devices[0] != e->device) return fail(SA_ERR_ARG, "communicator is on device %d, engine on %d", c->devices[0], e->device);
+  if (c->sim >= 0) {
+    if (c->sim != e->sim) return fail(SA_ERR_ARG, "engine has similarity %d, the communicator's ranks %d", e->sim, c->sim);
+    return SA_OK;
+  }
+  // First search on this communicator (a collective, like the search itself): all-gather every rank's similarity once;
+  // shards ranked under different similarities cannot be merged.
+  SA_ON_DEVICE(e->device);
+  int* d = nullptr;
+  SA_CUDA(cudaMalloc(&d, sizeof(int) * (c->n_ranks + 1)));
+  std::vector<int> got(c->n_ranks, -1);
+  cudaError_t ce = cudaMemcpy(d + c->n_ranks, &e->sim, sizeof(int), cudaMemcpyHostToDevice);
+  ncclResult_t nr = ncclSuccess;
+  if (ce == cudaSuccess) nr = g_nccl.AllGather(d + c->n_ranks, d, 1, ncclInt32, c->comms[0], e->own_stream);
+  if (ce == cudaSuccess && nr == ncclSuccess) ce = cudaStreamSynchronize(e->own_stream);
+  if (ce == cudaSuccess && nr == ncclSuccess) ce = cudaMemcpy(got.data(), d, sizeof(int) * c->n_ranks, cudaMemcpyDeviceToHost);
+  cudaFree(d);
+  if (nr != ncclSuccess) return fail(SA_ERR_COMM, "similarity all-gather failed: %s", g_nccl.GetErrorString(nr));
+  if (ce != cudaSuccess) return fail(SA_ERR_CUDA, "similarity all-gather: %s", cudaGetErrorString(ce));
+  for (int r = 0; r < c->n_ranks; ++r)
+    if (got[r] != e->sim) return fail(SA_ERR_ARG, "rank %d has similarity %d, this rank %d", r, got[r], e->sim);
+  c->sim = e->sim;
   return SA_OK;
 }
 }  // namespace
@@ -1240,6 +1326,8 @@ int sa_gather_merge_submit(sa_comm* c, sa_engine* const* engines, int slot, cons
     if (rc) return rc;
     if (engines[g]->device != c->devices[g])
       return fail(SA_ERR_ARG, "engine %d is on device %d, communicator rank %d on %d", g, engines[g]->device, g, c->devices[g]);
+    if (engines[g]->sim != engines[0]->sim)
+      return fail(SA_ERR_ARG, "engine %d has similarity %d, engine 0 has %d", g, engines[g]->sim, engines[0]->sim);
   }
   // every GPU gets the query block and runs the identical single-GPU path; the collectives of all local ranks are
   // issued inside one NCCL group (a single thread drives all devices)
@@ -1429,6 +1517,14 @@ int sa_get_info(const sa_engine* e, const char* name, int64_t* value) {
   else if (!strcmp(name, "dbg_times_ptr")) *value = static_cast<int64_t>(reinterpret_cast<uintptr_t>(e->dbg_times));
   else if (!strcmp(name, "last_fix_entries")) *value = e->last_fix_entries;
   else if (!strcmp(name, "eps_rel_e12")) *value = static_cast<int64_t>(static_cast<double>(scan_eps_rel(e->dim)) * 1e12);
+  else if (!strcmp(name, "similarity")) *value = e->sim;
+  else if (!strcmp(name, "cmax_bits")) {
+    unsigned bits = 0;
+    DeviceGuard dg(e->device);
+    if (cudaMemcpy(&bits, e->cmax, sizeof bits, cudaMemcpyDeviceToHost) != cudaSuccess)
+      return fail(SA_ERR_CUDA, "reading cmax failed");
+    *value = bits;
+  }
   else return fail(SA_ERR_ARG, "unknown info '%s'", name);
   return SA_OK;
 }
@@ -1460,7 +1556,7 @@ int sa_debug_tile_dots(sa_engine* e, const void* q_bf16_dev, int nq, int tile, i
   rc = encode_rows_map(&tq, q_bf16_dev, static_cast<uint64_t>(nq), e->dim, sa::kBlockM);
   if (rc) return rc;
   sa::ScanParams sp = {};
-  sp.inv_norm = e->inv_norm;
+  sp.row_term = e->row_term;
   sp.n_rows = e->n_rows;
   sp.nq = nq;
   sp.num_kb = e->dim / sa::kBlockK;
@@ -1481,7 +1577,7 @@ int sa_debug_tile_dots(sa_engine* e, const void* q_bf16_dev, int nq, int tile, i
   sp.dbg_times = nullptr;
   sp.dbg_dots = out_dots_dev;
   sp.dbg_tile = tile;
-  return launch_scan_dispatch(cta_group, 16, sa::kModeDots, tq, e->tmap_c[cta_group - 1], sp, nqb * cta_group,
+  return launch_scan_dispatch(cta_group, 16, sa::kModeDots, sa::kEpiMul, tq, e->tmap_c[cta_group - 1], sp, nqb * cta_group,
                               reinterpret_cast<cudaStream_t>(stream));
 }
 

@@ -44,7 +44,35 @@ __device__ __forceinline__ double warp_sum(double v) {
   return v;
 }
 
-// inv_norm[r] = 1/sqrt(sum_j row[r][j]^2) over the stored bf16 values, 0 for an all-zero row.
+// Similarity of an index (SA_SIM_* of sa_api.h).  The row term w[r] the scan combines with its accumulator:
+//   cosine      1/|c|        0 for an all-zero row (never returned) or a tombstone
+//   dotProduct  1            0 for a tombstone (an all-zero row is a live row scoring 0)
+//   euclidean   |c|^2 / 2    -1 for a tombstone (an all-zero row is a live row at distance |q|)
+// Internally every kernel ranks by a float64 value where larger is better: cosine, <q,c>, and -|q - c|.
+constexpr int kSimCos = 0;
+constexpr int kSimDot = 1;
+constexpr int kSimEuc = 2;
+
+// Row term of a live row from its float64 sum of squares (dotProduct, euclidean); cosine keeps its fp32 path below.
+// |c|^2 is summed in fp64 and rounded once: an fp32 sum of 1536 squares is off by ~1e-4 relative, the size of the whole
+// certificate band.  Also returns (through cmax) an upper bound on the row's norm: sqrt in fp64, nudged up, rounded up.
+template <int kSim>
+__device__ __forceinline__ float row_term_f64(double ss) {
+  return kSim == kSimEuc ? __double2float_rn(0.5 * ss) : 1.0f;
+}
+__device__ __forceinline__ unsigned norm_bound_bits(double ss) {
+  return __float_as_uint(__double2float_ru(sqrt(ss) * (1.0 + 0x1p-40)));
+}
+// Raise the device scalar Cmax (float bits; non-negative floats order like their bits) by the largest bound of a block.
+__device__ __forceinline__ void block_raise_cmax(unsigned* cmax, unsigned* blk_max, unsigned mine, bool active) {
+  if (threadIdx.x == 0) *blk_max = 0u;
+  __syncthreads();
+  if (active) atomicMax(blk_max, mine);
+  __syncthreads();
+  if (threadIdx.x == 0 && *blk_max != 0u) atomicMax(cmax, *blk_max);
+}
+
+// inv_norm[r] = 1/sqrt(sum_j row[r][j]^2) over the stored bf16 values, 0 for an all-zero row (cosine).
 // One warp per row, 16-byte loads (dim % 8 == 0).
 __global__ void sa_rownorm_kernel(const uint16_t* __restrict__ rows, float* __restrict__ inv_norm, long long first,
                                   long long n, int dim) {
@@ -67,7 +95,42 @@ __global__ void sa_rownorm_kernel(const uint16_t* __restrict__ rows, float* __re
   if (lane == 0) inv_norm[first + w] = ss > 0.f ? 1.0f / sqrtf(ss) : 0.f;
 }
 
-// dst_bf16[r][:] = RNE(src_f32[r][:]); optionally also inv_norm[r] (corpus ingest).  One warp per row.
+// fp64 sum of squares of one bf16 row (squares of bf16 values are exact in fp32), one warp, every lane gets it.
+__device__ __forceinline__ double row_ss_f64(const uint4* __restrict__ src, int nvec, int lane) {
+  double ss = 0.0;
+  for (int i = lane; i < nvec; i += 32) {
+    const uint4 x = __ldg(src + i);
+    const uint32_t u[4] = {x.x, x.y, x.z, x.w};
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const float a = bf16_bits_to_f32(u[k] & 0xffffu), b = bf16_bits_to_f32(u[k] >> 16);
+      ss += static_cast<double>(a * a);
+      ss += static_cast<double>(b * b);
+    }
+  }
+  return warp_sum(ss);
+}
+
+// dotProduct / euclidean form of sa_rownorm_kernel: w[r] = row_term_f64 of the row, and Cmax raised to cover it.
+// first < 0: recompute Cmax only (sa_corpus_bind), leaving w untouched.  One warp per row.
+template <int kSim>
+__global__ void sa_rowterm_kernel(const uint16_t* __restrict__ rows, float* __restrict__ w_out, long long first,
+                                  long long n, int dim, unsigned* __restrict__ cmax) {
+  __shared__ unsigned blk_max;
+  const long long w = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  const bool active = w < n;
+  unsigned nb = 0u;
+  if (active) {
+    const long long r = (first < 0 ? 0 : first) + w;
+    const double ss = row_ss_f64(reinterpret_cast<const uint4*>(rows + r * dim), dim / 8, lane);
+    if (lane == 0 && first >= 0) w_out[r] = row_term_f64<kSim>(ss);
+    nb = norm_bound_bits(ss);
+  }
+  block_raise_cmax(cmax, &blk_max, nb, active && lane == 0);
+}
+
+// dst_bf16[r][:] = RNE(src_f32[r][:]); optionally also inv_norm[r] (corpus ingest, cosine).  One warp per row.
 __global__ void sa_convert_rows_kernel(const float* __restrict__ src, uint16_t* __restrict__ dst,
                                        float* __restrict__ inv_norm, long long n, int dim) {
   const long long w = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
@@ -94,6 +157,38 @@ __global__ void sa_convert_rows_kernel(const float* __restrict__ src, uint16_t* 
   }
 }
 
+// dotProduct / euclidean corpus ingest: dst_bf16[r][:] = RNE(src_f32[r][:]), w[r] = row_term_f64, Cmax raised.
+template <int kSim>
+__global__ void sa_convert_rows_term_kernel(const float* __restrict__ src, uint16_t* __restrict__ dst,
+                                            float* __restrict__ w_out, long long n, int dim, unsigned* __restrict__ cmax) {
+  __shared__ unsigned blk_max;
+  const long long w = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  const bool active = w < n;
+  unsigned nb = 0u;
+  if (active) {
+    const float4* s = reinterpret_cast<const float4*>(src + w * dim);
+    uint2* d = reinterpret_cast<uint2*>(dst + w * dim);
+    double ss = 0.0;
+    for (int i = lane; i < dim / 4; i += 32) {
+      const float4 x = __ldg(s + i);
+      const uint32_t b0 = f32_to_bf16_bits(x.x), b1 = f32_to_bf16_bits(x.y), b2 = f32_to_bf16_bits(x.z),
+                     b3 = f32_to_bf16_bits(x.w);
+      d[i] = make_uint2(b0 | (b1 << 16), b2 | (b3 << 16));
+      const float r0 = bf16_bits_to_f32(b0), r1 = bf16_bits_to_f32(b1), r2 = bf16_bits_to_f32(b2),
+                  r3 = bf16_bits_to_f32(b3);
+      ss += static_cast<double>(r0 * r0);
+      ss += static_cast<double>(r1 * r1);
+      ss += static_cast<double>(r2 * r2);
+      ss += static_cast<double>(r3 * r3);
+    }
+    ss = warp_sum(ss);
+    if (lane == 0) w_out[w] = row_term_f64<kSim>(ss);
+    nb = norm_bound_bits(ss);
+  }
+  block_raise_cmax(cmax, &blk_max, nb, active && lane == 0);
+}
+
 // Order-preserving map: (score desc, row asc)  <=>  key desc.
 __host__ __device__ __forceinline__ unsigned long long make_key(float s, int row) {
   uint32_t u = aux_f32_bits(s);
@@ -105,15 +200,16 @@ __host__ __device__ __forceinline__ int key_row(unsigned long long k) { return s
 // ------------------------------------------------------------------------------------------------------------------
 // Stage 2 of the search: merge the per-lane candidate lists of one query, certify, re-score exactly.
 //
-// Notation (all in the scan's "approximate units": a(r) = fp32_accumulate(q . c_r) * fl(1/|c_r|), no 1/|q| factor;
-// the exact value in the same units is e(r) = <q, c_r> / |c_r| = cos(q, c_r) * |q|):
-//   eps     bound on |a(r) - e(r)|, = eps_rel * |q|  (eps_rel from the engine: ~dim * 2^-23, DESIGN.md section 4.2)
+// Notation (all in the scan's "approximate units": a(r) = fp32_accumulate(q . c_r) * fl(w_r) (euclidean: - fl(w_r)), no
+// 1/|q| factor; the exact value in the same units is e(r) = <q, c_r> / |c_r| = cos(q, c_r) * |q| for cosine, <q, c_r>
+// for dotProduct, <q, c_r> - |c_r|^2 / 2 = (|q|^2 - |q - c_r|^2) / 2 for euclidean):
+//   eps     bound on |a(r) - e(r)|, cert_eps below (eps_rel from the engine: ~dim * 2^-23, DESIGN.md section 4.2)
 //   U       union of the TL lane lists of the query;  drop_l >= a(r) for every row r of lane l that is not in U
 //   A_k     k-th largest a over U
 // Claim.  Let band = A_k - 2 eps.  If drop_l < band for every lane l, then every row outside U has a < band, A_k is the
 // k-th largest a over the WHOLE corpus, and every row of the exact top-k has a >= T - eps >= A_k - 2 eps = band (T = k-th
 // largest e; T >= A_k - eps because the k rows with a >= A_k have e >= A_k - eps).  So the exact top-k is contained in
-// {r in U : a(r) >= band}; re-scoring that set in float64 and sorting by (cosine desc, row asc) IS the brute-force answer.
+// {r in U : a(r) >= band}; re-scoring that set in float64 and sorting by (value desc, row asc) IS the brute-force answer.
 // A lane with drop_l >= band ("ambiguous") may have discarded such a row: the query then gets one work item per ambiguous
 // lane for the exact fallback scan (sa_fixup_kernel), which re-reads only those lanes' tiles.
 // ------------------------------------------------------------------------------------------------------------------
@@ -123,6 +219,7 @@ struct FixEntry {
 };
 struct FixQuery {
   double qq;    // |q|^2
+  float eps;    // the certificate's bound |a - e| for this query (cert_eps)
   float band;   // prefilter threshold in approximate units (-inf: everything is re-scored)
   int lock;     // spin lock of the query's result list during the fallback scan (0 = free)
 };
@@ -141,8 +238,10 @@ struct MergeParams {
   int tl_count;
   int unit_map;             // same mapping switch as ScanParams::unit_map
   int q0;                   // index of this launch's first query within the whole search
-  float eps_rel;            // |a - e| <= eps_rel * |q|
-  double* res64;            // [nq][k] this launch's slice of the search's internal result: cosine (float64) ...
+  float eps_rel;            // relative accumulation bound of the scan (cert_eps)
+  int sim;                  // kSimCos / kSimDot / kSimEuc
+  const unsigned* cmax;     // device scalar (float bits): upper bound on |c| over the committed rows (not cosine)
+  double* res64;            // [nq][k] this launch's slice of the search's internal result: value (float64) ...
   int* residx;              // ... and shard-local row, -1 / -inf when fewer than k rows qualify
   FixEntry* fix_entries;    // work queue of the fallback scan
   int* fix_count;           // zero at the start of a search
@@ -162,11 +261,14 @@ __device__ __forceinline__ float key_score(unsigned long long k) {
   return aux_bits_f32((u & 0x80000000u) ? (u & 0x7fffffffu) : ~u);
 }
 
-// Exact cosine of (query, corpus row), one warp: bf16 x bf16 products are exact in fp32; sums of products and of squares
-// in float64, lane-strided then a butterfly.  Every lane returns the same value.  Used by the merge kernel AND the
-// fallback scan, so the two produce bit-identical cosines for the same pair.
-__device__ __forceinline__ double exact_cosine_warp(const uint4* __restrict__ qv, const uint4* __restrict__ cv, int nvec,
-                                                    double qq, int lane) {
+// Exact internal value of (query, corpus row), one warp: bf16 x bf16 products are exact in fp32; sums of products and of
+// squares in float64, lane-strided then a butterfly.  Every lane returns the same value.  Used by the merge kernel AND
+// the fallback scan, so the two produce bit-identical values for the same pair.  Larger is better:
+//   cosine      <q,c> / sqrt(|q|^2 |c|^2)   (0 when either is all-zero)
+//   dotProduct  <q,c>
+//   euclidean   -sqrt(max(d2, 0)),  d2 = (|q|^2 - 2 <q,c>) + |c|^2   -- one fixed formula, the oracle's too
+__device__ __forceinline__ double exact_value_warp(const uint4* __restrict__ qv, const uint4* __restrict__ cv, int nvec,
+                                                   double qq, int lane, int sim) {
   double dot = 0.0, dd = 0.0;
   for (int i = lane; i < nvec; i += 32) {
     const uint4 x = __ldg(qv + i);
@@ -184,9 +286,37 @@ __device__ __forceinline__ double exact_cosine_warp(const uint4* __restrict__ qv
     }
   }
   dot = warp_sum(dot);
+  if (sim == kSimDot) return dot;
   dd = warp_sum(dd);
+  if (sim == kSimEuc) {
+    const double d2 = __dadd_rn(__dsub_rn(qq, 2.0 * dot), dd);  // no contraction: the oracle evaluates the same two ops
+    return -sqrt(d2 > 0.0 ? d2 : 0.0);
+  }
   const double den = qq * dd;
   return den > 0.0 ? dot / sqrt(den) : 0.0;
+}
+
+// The certificate's bound eps >= |a(r) - e(r)| for every committed row r, rounded up (DESIGN.md section 4.2).
+//   cosine      eps_rel |q|                                    (the row's norm cancels against w = 1/|c|)
+//   dotProduct  eps_rel |q| Cmax                               (|acc - <q,c>| <= dim 2^-23 |q| |c|)
+//   euclidean   (eps_rel + 2^-23) |q| Cmax + 2^-23 Cmax^2 + 2^-50 |q|^2
+//               (accumulation as above; w rounded once from fp64: 2^-24 |c|^2/2; the subtraction: 2^-24 (|acc| + w);
+//                the last term covers the fallback's fp64 conversion of a distance into these units)
+// Cmax is an upper bound on the committed rows' norms, kept on the device: reading it costs the search no host sync.
+__device__ __forceinline__ float cert_eps(int sim, double qq, float eps_rel, const unsigned* cmax) {
+  const double qn = sqrt(qq);
+  if (sim == kSimCos) return __double2float_ru(qn * static_cast<double>(eps_rel));
+  const double cm = static_cast<double>(__uint_as_float(*cmax));
+  if (sim == kSimDot) return __double2float_ru(qn * cm * static_cast<double>(eps_rel) * (1.0 + 0x1p-40));
+  const double u = 0x1p-23;
+  return __double2float_ru(((static_cast<double>(eps_rel) + u) * qn * cm + u * cm * cm + 0x1p-50 * qq) * (1.0 + 0x1p-40));
+}
+
+// An exact internal value (exact_value_warp) in the scan's units, rounded down (towards a wider prefilter).
+__device__ __forceinline__ float value_to_scan_rd(int sim, double v, double qq) {
+  if (sim == kSimCos) return __double2float_rd(v * sqrt(qq));
+  if (sim == kSimDot) return __double2float_rd(v);
+  return __double2float_rd(0.5 * (qq - v * v));  // v = -d: (|q|^2 - d^2) / 2
 }
 __device__ __forceinline__ double query_norm2_warp(const uint4* __restrict__ qv, int nvec, int lane) {
   double qq = 0.0;
@@ -203,7 +333,7 @@ __device__ __forceinline__ double query_norm2_warp(const uint4* __restrict__ qv,
   return warp_sum(qq);
 }
 
-// (cosine desc, row asc): does (c1, r1) come before (c2, r2)?
+// (value desc, row asc): does (c1, r1) come before (c2, r2)?
 __host__ __device__ __forceinline__ bool result_before(double c1, int r1, double c2, int r2) {
   return c1 > c2 || (c1 == c2 && r1 < r2);
 }
@@ -283,7 +413,7 @@ __global__ void __launch_bounds__(kMergeThreads) sa_merge_rescore_kernel(const M
   }
   const double qq = qq_s;
   // eps and band, rounded towards "wider"
-  const float eps = __double2float_ru(sqrt(qq) * static_cast<double>(p.eps_rel));
+  const float eps = cert_eps(p.sim, qq, p.eps_rel, p.cmax);
   const float band = (kth != 0ull) ? __fsub_rd(key_score(kth), __fmul_ru(2.0f, eps)) : -INFINITY;
 
   // ---- ambiguous lanes, and the band candidates of U
@@ -305,7 +435,7 @@ __global__ void __launch_bounds__(kMergeThreads) sa_merge_rescore_kernel(const M
   for (int c = warp; c < nsel; c += kMergeWarps) {
     const int crow = key_row(sel[c]);
     const uint4* cv = reinterpret_cast<const uint4*>(p.corpus + static_cast<size_t>(crow) * p.dim);
-    const double v = exact_cosine_warp(qv, cv, nvec, qq, lane);
+    const double v = exact_value_warp(qv, cv, nvec, qq, lane, p.sim);
     if (lane == 0) cs[c] = v;
   }
   __syncthreads();
@@ -338,6 +468,7 @@ __global__ void __launch_bounds__(kMergeThreads) sa_merge_rescore_kernel(const M
     if (tid == 0) {
       FixQuery fq;
       fq.qq = qq;
+      fq.eps = eps;
       fq.band = band;
       fq.lock = 0;
       p.fix_query[p.q0 + q] = fq;
@@ -351,13 +482,13 @@ __global__ void __launch_bounds__(kMergeThreads) sa_merge_rescore_kernel(const M
 // output arrays and re-zeroes the scan's scratch for the next search.
 //
 // Work item = (queue entry, chunk of kFixChunkTiles tiles of that lane).  A CTA stages the query (fp32) in shared memory;
-// each warp walks rows: fp32 dot (CUDA cores) * 1/|c| -> a'(r), whose error is far inside eps; rows with a' >= max(band,
-// current k-th exact cosine in approximate units - eps) are re-scored exactly and inserted into the WARP's own list (no
+// each warp walks rows: fp32 dot (CUDA cores) * w (euclidean: - w) -> a'(r), whose error is inside eps; rows with a' >=
+// max(band, current k-th exact value in approximate units - eps) are re-scored exactly and inserted into the WARP's own list (no
 // sharing between warps, so no locks in shared memory); at the end of the item one thread folds the warps' lists into the
 // query's result under the query's lock (rows already present are skipped).  The last CTA to finish finalises.
 // ------------------------------------------------------------------------------------------------------------------
 struct PackedHit {
-  double score;       // cosine, float64
+  double score;       // the returned value, float64: cosine, dot product or Euclidean distance
   long long row;      // global row (shard offset applied), -1 = none
 };
 
@@ -367,7 +498,7 @@ struct FixParams {
   int* done_count;
   FixQuery* fix_query;
   const uint16_t* corpus;
-  const float* inv_norm;
+  const float* row_term;
   const uint16_t* queries;  // [nq][dim] the whole search
   long long n_rows;
   int num_tiles;
@@ -375,11 +506,11 @@ struct FixParams {
   int nq;
   int k;
   int chunks_per_entry;     // ceil(max tiles per lane / kFixChunkTiles)
-  float eps_rel;
+  int sim;                  // kSimCos / kSimDot / kSimEuc
   double* res64;            // [nq][k] internal result (read / updated here)
   int* residx;
-  // finalisation
-  float* out_score;         // [nq][k] fp32 cosine
+  // finalisation: the internal value becomes the returned one (euclidean: the distance, -v)
+  float* out_score;         // [nq][k] fp32 value
   int* out_idx;             // [nq][k] shard-local row
   double* out_score64;      // optional
   PackedHit* out_packed;    // optional: (cosine f64, global row) for the cross-shard exchange
@@ -399,7 +530,7 @@ constexpr int kFixMaxK = 32;
 __device__ __forceinline__ void fix_finalize(const FixParams& p, int first, int stride) {
   const int total = p.nq * p.k;
   for (int i = first; i < total; i += stride) {
-    const double s = p.res64[i];
+    const double s = p.sim == kSimEuc ? -p.res64[i] : p.res64[i];  // empty slots: -inf -> +inf for distances
     const int r = p.residx[i];
     p.out_score[i] = static_cast<float>(s);
     p.out_idx[i] = r;
@@ -461,8 +592,7 @@ __global__ void __launch_bounds__(kFixThreads) sa_fixup_kernel(const FixParams p
     if (t_first >= p.num_tiles) continue;  // block-uniform
     FixQuery* fq = p.fix_query + en.q;
     const double qq = fq->qq;
-    const double qn = sqrt(qq);
-    const float eps = __double2float_ru(qn * static_cast<double>(p.eps_rel));
+    const float eps = fq->eps;
     volatile double* g_cos = p.res64 + static_cast<size_t>(en.q) * p.k;
     volatile int* g_row = p.residx + static_cast<size_t>(en.q) * p.k;
     const uint4* qv = reinterpret_cast<const uint4*>(p.queries + static_cast<size_t>(en.q) * p.dim);
@@ -480,16 +610,16 @@ __global__ void __launch_bounds__(kFixThreads) sa_fixup_kernel(const FixParams p
       l_row[i / kFixMaxK][i % kFixMaxK] = -1;
     }
     if (tid == 0) {
-      // prefilter threshold: the band of the merge kernel, tightened by the k-th exact cosine found so far
+      // prefilter threshold: the band of the merge kernel, tightened by the k-th exact value found so far
       float thr = fq->band;
       const int rk = g_row[p.k - 1];
-      if (rk >= 0) thr = fmaxf(thr, __fsub_rd(__double2float_rd(g_cos[p.k - 1] * qn), eps));
+      if (rk >= 0) thr = fmaxf(thr, __fsub_rd(value_to_scan_rd(p.sim, g_cos[p.k - 1], qq), eps));
       thr0_s = thr;
     }
     __syncthreads();
     float thr = thr0_s;           // per warp from here on: tightened by the warp's own list (uniform across its lanes)
     double* wc = l_cos[warp];
-    int* wr = l_row[warp];
+    int* wrow = l_row[warp];
 
     for (int ti = 0; ti < kFixChunkTiles; ++ti) {
       const int t = t_first + ti * TL;
@@ -497,8 +627,8 @@ __global__ void __launch_bounds__(kFixThreads) sa_fixup_kernel(const FixParams p
       for (int rr = warp; rr < 256; rr += kWarps) {
         const long long r = static_cast<long long>(t) * 256 + rr;
         if (r >= p.n_rows) break;
-        const float inv = __ldg(p.inv_norm + r);
-        if (!(inv > 0.f)) continue;  // all-zero rows are never returned
+        const float wr = __ldg(p.row_term + r);
+        if (p.sim == kSimEuc ? !(wr >= 0.f) : !(wr > 0.f)) continue;  // rows that are not live are never returned
         const uint4* cv = reinterpret_cast<const uint4*>(p.corpus + static_cast<size_t>(r) * p.dim);
         float acc = 0.f;
         for (int i = lane; i < nvec; i += 32) {
@@ -514,13 +644,13 @@ __global__ void __launch_bounds__(kFixThreads) sa_fixup_kernel(const FixParams p
           acc = fmaf(b.w, bf16_bits_to_f32(y.w >> 16), acc);
         }
         acc = warp_sum(acc);
-        const float ap = acc * inv;
+        const float ap = p.sim == kSimEuc ? acc - wr : acc * wr;
         if (!(ap >= thr)) continue;  // warp-uniform (every lane holds the same sum)
-        const double c = exact_cosine_warp(qv, cv, nvec, qq, lane);
+        const double c = exact_value_warp(qv, cv, nvec, qq, lane, p.sim);
         float nt = thr;
         if (lane == 0) {
-          fix_list_insert(wc, wr, p.k, c, static_cast<int>(r));
-          if (wr[p.k - 1] >= 0) nt = fmaxf(thr, __fsub_rd(__double2float_rd(wc[p.k - 1] * qn), eps));
+          fix_list_insert(wc, wrow, p.k, c, static_cast<int>(r));
+          if (wrow[p.k - 1] >= 0) nt = fmaxf(thr, __fsub_rd(value_to_scan_rd(p.sim, wc[p.k - 1], qq), eps));
         }
         thr = __shfl_sync(0xffffffffu, nt, 0);
       }
@@ -559,14 +689,15 @@ __global__ void __launch_bounds__(kFixThreads) sa_fixup_kernel(const FixParams p
 }
 
 // After the all-gather of the packed per-shard results: per query, merge G shard lists of k (already sorted, global
-// rows) into the global top-k by (cosine desc, global row asc).  One warp per query, lane g holds the head of shard g's
+// rows) into the global top-k by (value desc, global row asc); asc = 1 (distances): by (value asc, global row asc).
+// The scores are negated on load and back on store when asc, so one "larger is better" loop serves both.  One warp per query, lane g holds the head of shard g's
 // list (G <= 32): k rounds of a warp arg-max, the winning lane advances.  The lists are first staged in shared memory
 // with coalesced 16-byte loads.
 constexpr int kMergePackedWarps = 4;
 constexpr int kMergePackedMaxK = 32;
 __global__ void __launch_bounds__(kMergePackedWarps * 32)
 sa_merge_packed_kernel(const PackedHit* __restrict__ hits, int n_shards, int nq, int k, float* __restrict__ out_score,
-                       long long* __restrict__ out_idx) {
+                       long long* __restrict__ out_idx, int asc) {
   __shared__ PackedHit stage[kMergePackedWarps][32 * kMergePackedMaxK / 4];  // n_shards * k <= 256 hits per query
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int q = blockIdx.x * kMergePackedWarps + warp;
@@ -584,7 +715,7 @@ sa_merge_packed_kernel(const PackedHit* __restrict__ hits, int n_shards, int nq,
     long long r = -1;
     if (lane < n_shards && head < k) {
       const PackedHit h = mine[lane * per + head];
-      s = h.score;
+      s = asc ? -h.score : h.score;
       r = h.row;
     }
     // warp arg-max by (score desc, row asc); lanes without a candidate carry r = -1
@@ -601,7 +732,7 @@ sa_merge_packed_kernel(const PackedHit* __restrict__ hits, int n_shards, int nq,
     if (r >= 0 && r == br) ++head;  // global rows are unique: exactly one lane advances
     if (lane == 0) {
       const size_t oo = static_cast<size_t>(q) * k + i;
-      out_score[oo] = br >= 0 ? static_cast<float>(bs) : -INFINITY;
+      out_score[oo] = br >= 0 ? static_cast<float>(asc ? -bs : bs) : (asc ? INFINITY : -INFINITY);
       out_idx[oo] = br;
     }
   }
@@ -609,7 +740,7 @@ sa_merge_packed_kernel(const PackedHit* __restrict__ hits, int n_shards, int nq,
 
 // The same merge for any number of shards (one thread per query); used when n_shards > 32 or n_shards * k > 256.
 __global__ void sa_merge_packed_serial_kernel(const PackedHit* __restrict__ hits, int n_shards, int nq, int k,
-                                              float* __restrict__ out_score, long long* __restrict__ out_idx) {
+                                              float* __restrict__ out_score, long long* __restrict__ out_idx, int asc) {
   const int q = blockIdx.x * blockDim.x + threadIdx.x;
   if (q >= nq) return;
   int head[64];
@@ -625,29 +756,30 @@ __global__ void sa_merge_packed_serial_kernel(const PackedHit* __restrict__ hits
         head[g] = k;
         continue;
       }
-      if (bg < 0 || h.score > bs || (h.score == bs && h.row < bi)) {
+      const double hs = asc ? -h.score : h.score;
+      if (bg < 0 || hs > bs || (hs == bs && h.row < bi)) {
         bg = g;
-        bs = h.score;
+        bs = hs;
         bi = h.row;
       }
     }
     const size_t oo = static_cast<size_t>(q) * k + i;
     if (bg >= 0) {
-      out_score[oo] = static_cast<float>(bs);
+      out_score[oo] = static_cast<float>(asc ? -bs : bs);
       out_idx[oo] = bi;
       ++head[bg];
     } else {
-      out_score[oo] = -INFINITY;
+      out_score[oo] = asc ? INFINITY : -INFINITY;
       out_idx[oo] = -1;
     }
   }
 }
 
 // After the all-gather: per query, merge G shard lists of k (already sorted, global row ids) into the
-// global top-k by (cosine desc, global row asc).  One thread per query; G*k <= a few hundred.
+// global top-k by (value desc, global row asc), or (value asc, ...) when asc.  One thread per query; G*k <= a few hundred.
 __global__ void sa_merge_shards_kernel(const double* __restrict__ score64, const long long* __restrict__ gidx,
                                        int n_shards, int nq, int k, float* __restrict__ out_score,
-                                       long long* __restrict__ out_idx) {
+                                       long long* __restrict__ out_idx, int asc) {
   const int q = blockIdx.x * blockDim.x + threadIdx.x;
   if (q >= nq) return;
   int head[64];
@@ -664,7 +796,7 @@ __global__ void sa_merge_shards_kernel(const double* __restrict__ score64, const
         head[g] = k;
         continue;
       }
-      const double s = score64[o];
+      const double s = asc ? -score64[o] : score64[o];
       if (bg < 0 || s > bs || (s == bs && ri < bi)) {
         bg = g;
         bs = s;
@@ -673,11 +805,11 @@ __global__ void sa_merge_shards_kernel(const double* __restrict__ score64, const
     }
     const size_t oo = static_cast<size_t>(q) * k + i;
     if (bg >= 0) {
-      out_score[oo] = static_cast<float>(bs);
+      out_score[oo] = static_cast<float>(asc ? -bs : bs);
       out_idx[oo] = bi;
       ++head[bg];
     } else {
-      out_score[oo] = -INFINITY;
+      out_score[oo] = asc ? INFINITY : -INFINITY;
       out_idx[oo] = -1;
     }
   }

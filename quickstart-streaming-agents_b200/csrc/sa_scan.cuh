@@ -4,7 +4,13 @@
 //
 //   TMA (SWIZZLE_128B tiles of the bf16 corpus and of the query block)  ->  smem ring
 //   wgmma  Q[64 x D] . C[128 x D]^T per consumer warpgroup, fp32 accumulators in registers
-//   epilogue: accumulators -> smem -> scale by the row's 1/|c| -> per-thread (thread == query) sorted register list
+//   epilogue: accumulators -> smem -> combine with the row's term w[r] -> per-thread (thread == query) sorted register list
+//
+// The row term w[r] and the epilogue make one kernel serve every similarity of the index (sa_api.h, SA_SIM_*):
+//   cosine      v = acc * w, w = 1/|c|     (0 = tombstone)         kEpi = kEpiMul
+//   dotProduct  v = acc * w, w = 1         (0 = tombstone)         kEpi = kEpiMul  (the cosine instantiations, unchanged)
+//   euclidean   v = acc - w, w = |c|^2 / 2 (negative = tombstone)  kEpi = kEpiSub
+// so v is always "larger is better": for euclidean v = <q,c> - |c|^2/2 = (|q|^2 - |q - c|^2) / 2.
 //
 // Nothing but the per-CTA candidate lists (kKL entries per query, plus one "dropped" bound per query) leaves the SM.
 //
@@ -15,7 +21,7 @@
 // same time (drift control below keeps it so): it crosses HBM once and is served from L2 to the others.
 //
 // Exactness contract with the merge kernel (sa_aux.cuh).  A thread's list holds the kKL best rows of its tile lane by
-// the scan's approximate score a = fp32_accumulate(q.c) * (1/|c|), and `drop` is an upper bound on the approximate
+// the scan's approximate score a = fp32_accumulate(q.c) * w (or - w), and `drop` is an upper bound on the approximate
 // score of every row of the lane that is NOT in the list (evicted, rejected by the own threshold, or rejected by the
 // bound shared between lanes).  The merge kernel turns (lists, drops) into either a certificate that the exactly
 // re-scored candidates contain the true top-k, or a work item for the exact fallback scan.
@@ -41,6 +47,10 @@ constexpr int kWinWarmTiles = 16;  // the window is read on every one of a lane'
 constexpr int kModeProd = 0;   // production
 constexpr int kModeDots = 1;   // test hook: also dump the raw accumulators of one tile
 constexpr int kModeProf = 2;   // profiling: per-role wait / busy cycle counters (ScanParams::prof)
+
+// kEpi of the scan kernel: how the accumulator and the row term combine (see the header comment)
+constexpr int kEpiMul = 0;     // v = acc * w; a row is live iff w > 0 (cosine, dotProduct)
+constexpr int kEpiSub = 1;     // v = acc - w; a row is live iff w >= 0 (euclidean)
 
 template <int kCG>
 struct ScanCfg {
@@ -70,7 +80,8 @@ struct ScanProf {
 };
 
 struct ScanParams {
-  const float* inv_norm;  // [capacity] 1/|row| over the bf16-rounded row, 0 for an all-zero row; 16-byte aligned
+  const float* row_term;  // [capacity] w[r] (cosine: 1/|row| over the bf16-rounded row, 0 for an all-zero row or a
+                          // tombstone; see kEpi for the others); 16-byte aligned
   long long n_rows;       // committed rows (epoch snapshot); rows >= n_rows are masked
   int nq;                 // queries covered by tmap_q
   int num_kb;             // D / 64
@@ -249,7 +260,7 @@ struct TopList {
 // as many rounds as its busiest lane needs (usually one or two), however the qualifying values are spread over the 32
 // rows; walking the rows group by group instead costs a round per group that ANY lane has a hit in, which during the
 // warm-up of a short scan (few tiles per lane) dominates the epilogue's time.
-template <int kKL>
+template <int kKL, int kEpi = kEpiMul>
 __host__ __device__ __forceinline__ bool chunk_process(TopList<kKL>& L, float (&v)[kChunk], const float (&w)[kChunk],
                                                        int row_base) {
   auto reduce = [&]() {
@@ -264,7 +275,12 @@ __host__ __device__ __forceinline__ bool chunk_process(TopList<kKL>& L, float (&
 #ifdef __CUDA_ARCH__
 #pragma unroll
 #endif
-  for (int i = 0; i < kChunk; ++i) v[i] *= w[i];
+  for (int i = 0; i < kChunk; ++i) {
+    if constexpr (kEpi == kEpiSub)
+      v[i] -= w[i];
+    else
+      v[i] *= w[i];
+  }
   float m = reduce();
   if (!(m > L.thr)) {
     L.drop = max_nn(L.drop, m);
@@ -299,7 +315,7 @@ __host__ __device__ __forceinline__ bool chunk_process(TopList<kKL>& L, float (&
 #ifdef __CUDACC__
 // Epilogue of one half tile: 128 columns of this thread's query row in the staging buffer -> scaled scores -> list.
 // `ic` is this warp's private 256-float scale vector of the tile in shared memory (broadcast reads).
-template <int kKL, int kMode>
+template <int kKL, int kMode, int kEpi>
 __device__ __forceinline__ int epilogue_half(TopList<kKL>& L, const float* srow, const float* ic, int row0,
                                              float* dbg_row) {
   int slow = 0;
@@ -326,13 +342,13 @@ __device__ __forceinline__ int epilogue_half(TopList<kKL>& L, const float* srow,
         for (int j = 0; j < kChunk; ++j) dbg_row[c * kChunk + j] = v[j];
       }
     }
-    slow += chunk_process<kKL>(L, v, w, row0 + c * kChunk) ? 1 : 0;
+    slow += chunk_process<kKL, kEpi>(L, v, w, row0 + c * kChunk) ? 1 : 0;
     __syncwarp();  // reconverge after the divergent insertion path
   }
   return slow;
 }
 
-template <int kCG, int kKL, int kMode>
+template <int kCG, int kKL, int kMode, int kEpi = kEpiMul>
 __global__ void __launch_bounds__(kScanThreads, 1)
 sa_scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_c,
                const ScanParams p) {
@@ -468,20 +484,22 @@ sa_scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant
     TopList<kKL> L;
     L.init((p.thr_shared != nullptr && own_query) ? p.thr_shared + query : nullptr);
 
-    // Scales of tile t: lane l fetches rows [8l, 8l+8) (two 16-byte loads), masks rows past the committed prefix
-    // and all-zero rows with NaN (NaN never compares greater than a threshold, so they cannot enter a list and
-    // are ignored by every max), and the warp shares them through its private smem vector.
+    // Row terms of tile t: lane l fetches rows [8l, 8l+8) (two 16-byte loads), masks rows past the committed prefix
+    // and rows that are not live (all-zero rows under cosine, tombstones) with NaN (NaN never compares greater than a
+    // threshold, so they cannot enter a list and are ignored by every max), and the warp shares them through its
+    // private smem vector.  Past the prefix the term reads as kPast, which every epilogue masks.
+    constexpr float kPast = (kEpi == kEpiSub) ? -1.f : 0.f;
     float4 nx0 = make_float4(0.f, 0.f, 0.f, 0.f), nx1 = nx0;
     auto fetch_ic = [&](int t) {
       const long long r0 = static_cast<long long>(t) * kBlockN + 8 * lane;
-      const float4* src = reinterpret_cast<const float4*>(p.inv_norm + r0);
+      const float4* src = reinterpret_cast<const float4*>(p.row_term + r0);
       if (r0 + 8 <= p.n_rows) {
         nx0 = __ldg(src);
         nx1 = __ldg(src + 1);
       } else {
         float x[8];
 #pragma unroll
-        for (int j = 0; j < 8; ++j) x[j] = (r0 + j < p.n_rows) ? __ldg(p.inv_norm + r0 + j) : 0.f;
+        for (int j = 0; j < 8; ++j) x[j] = (r0 + j < p.n_rows) ? __ldg(p.row_term + r0 + j) : kPast;
         nx0 = make_float4(x[0], x[1], x[2], x[3]);
         nx1 = make_float4(x[4], x[5], x[6], x[7]);
       }
@@ -513,7 +531,12 @@ sa_scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant
         }
         L.apply_shared(L.nxt_key);
         const float qnan = __int_as_float(0x7fc00000);
-        auto sc = [&](float x) { return x > 0.f ? x : qnan; };
+        auto sc = [&](float x) {
+          if constexpr (kEpi == kEpiSub)
+            return x >= 0.f ? x : qnan;
+          else
+            return x > 0.f ? x : qnan;
+        };
         float4* dst = reinterpret_cast<float4*>(ic + 8 * lane);
         dst[0] = make_float4(sc(nx0.x), sc(nx0.y), sc(nx0.z), sc(nx0.w));
         dst[1] = make_float4(sc(nx1.x), sc(nx1.y), sc(nx1.z), sc(nx1.w));
@@ -583,7 +606,7 @@ sa_scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant
         long long c2 = 0;
         if constexpr (kProf) c2 = clock64();
         if (epi)
-          slow += epilogue_half<kKL, kMode>(L, stg + wt * kStagingLd, ic + h * kHalfN, t * kBlockN + h * kHalfN,
+          slow += epilogue_half<kKL, kMode, kEpi>(L, stg + wt * kStagingLd, ic + h * kHalfN, t * kBlockN + h * kHalfN,
                                             dbg_row != nullptr ? dbg_row + h * kHalfN : nullptr);
         if constexpr (kProf) {
           w_mma += c1 - c0;

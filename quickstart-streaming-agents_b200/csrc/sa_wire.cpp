@@ -415,6 +415,7 @@ int sa_wire_encode_search_results(int n, int k, int n_out, uint32_t schema_id, c
       p += len;
       double s = static_cast<double>(score[static_cast<size_t>(i) * k + j]);
       if (score_mode == 1) s = 0.5 * (1.0 + s);
+      else if (score_mode == 2) s = 1.0 / (1.0 + s);
       *p++ = 2;
       memcpy(p, &s, 8);
       p += 8;

@@ -46,12 +46,19 @@ def pinned_array(shape, dtype=np.float32) -> np.ndarray:
 
 
 class VectorIndex:
-    """A row shard of the corpus resident in HBM: bf16 rows [capacity, dim] + fp32 inverse norms [capacity]."""
+    """A row shard of the corpus resident in HBM: bf16 rows [capacity, dim] + one fp32 row term per row [capacity].
+
+    ``similarity`` is the Atlas index setting, fixed at creation: "cosine" (default), "dotProduct" or "euclidean"
+    (include/sa_api.h, SA_SIM_*).  Scores are cosines, dot products or Euclidean distances accordingly; results are
+    ordered best first (ascending distance for "euclidean").  ``inv_norm`` holds the row terms: 1/|c| for cosine, 1 for
+    dotProduct, |c|^2/2 for euclidean."""
 
     def __init__(self, dim: int = 1536, capacity: int = 1 << 20, max_batch: int = 1024, max_k: int = 10,
-                 device: int | None = None):
+                 device: int | None = None, similarity: str = "cosine"):
+        sim = capi.similarity_code(similarity)
         if not torch.cuda.is_available():
             raise RuntimeError("VectorIndex needs a CUDA device (H100, sm_90a); there is no CPU fallback")
+        self.similarity = similarity
         self.lib = capi.load()
         self.device = torch.cuda.current_device() if device is None else int(device)
         self.dim, self.capacity, self.max_batch, self.max_k = int(dim), int(capacity), int(max_batch), int(max_k)
@@ -60,8 +67,8 @@ class VectorIndex:
         self.rows = torch.empty((self.capacity, self.dim), dtype=torch.bfloat16, device=dev)
         self.inv_norm = torch.zeros((self.capacity,), dtype=torch.float32, device=dev)
         h = C.c_void_p()
-        capi.check(self.lib.sa_engine_create(C.byref(h), self.device, self.dim, self.capacity, self.max_batch,
-                                             self.max_k), "sa_engine_create")
+        capi.check(self.lib.sa_engine_create_sim(C.byref(h), self.device, self.dim, self.capacity, self.max_batch,
+                                                 self.max_k, sim), "sa_engine_create_sim")
         self._h = h
         self._inflight = {}
         capi.check(self.lib.sa_corpus_bind(self._h, self.rows.data_ptr(), self.inv_norm.data_ptr(), 0),
@@ -133,7 +140,8 @@ class VectorIndex:
 
     # ------------------------------------------------------------------ checkpoint / resume
     def snapshot(self, path: str) -> int:
-        """Write the committed rows (bf16 bits) and their inverse norms to ``path`` (.npz).  Returns the row count.
+        """Write the committed rows (bf16 bits), their row terms and the similarity to ``path`` (.npz).  Returns the
+        row count.
         (The reference leaves corpus durability to Atlas; here a snapshot + the consumer-group offsets are the
         checkpoint, and replaying `documents_embed` from offset 0 is the fallback.)"""
         n = len(self)
@@ -143,17 +151,23 @@ class VectorIndex:
         path = path if path.endswith(".npz") else path + ".npz"
         tmp = path + ".tmp"
         with open(tmp, "wb") as f:                       # written under a temporary name, then renamed: never half a file
-            np.savez(f, rows=bits, inv_norm=self.inv_norm[:n].cpu().numpy(), dim=np.int64(self.dim))
+            np.savez(f, rows=bits, inv_norm=self.inv_norm[:n].cpu().numpy(), dim=np.int64(self.dim),
+                     similarity=np.str_(self.similarity))
             f.flush()
             os.fsync(f.fileno())
         os.replace(tmp, path)
         return n
 
     def restore(self, path: str) -> int:
-        """Load a snapshot written by ``snapshot`` into this (empty or not) index, replacing its contents."""
+        """Load a snapshot written by ``snapshot`` into this (empty or not) index, replacing its contents.  A snapshot
+        without a recorded similarity is a cosine one; a snapshot of another similarity is refused (its row terms and
+        its rankings mean something else)."""
         z = np.load(path if path.endswith(".npz") else path + ".npz")
         if int(z["dim"]) != self.dim:
             raise ValueError(f"snapshot has dim {int(z['dim'])}, index has {self.dim}")
+        snap_sim = str(z["similarity"]) if "similarity" in z.files else "cosine"
+        if snap_sim != self.similarity:
+            raise ValueError(f"snapshot has similarity {snap_sim!r}, index has {self.similarity!r}")
         bits, inv = z["rows"], z["inv_norm"]
         n = bits.shape[0]
         if n > self.capacity:
@@ -166,12 +180,13 @@ class VectorIndex:
         return n
 
     def delete_rows(self, rows) -> None:
-        """Tombstone rows: zero the stored vector and its inverse norm -- all-zero rows are never returned."""
+        """Tombstone rows: zero the stored vector and write the tombstone row term (0, or -1 for euclidean, where a
+        zero vector is a live row) -- tombstoned rows are never returned."""
         if len(rows) == 0:
             return
         ix = torch.as_tensor(list(rows), dtype=torch.long, device=self.rows.device)
         self.rows.index_fill_(0, ix, 0)
-        self.inv_norm.index_fill_(0, ix, 0)
+        self.inv_norm.index_fill_(0, ix, -1.0 if self.similarity == "euclidean" else 0.0)
 
     def commit(self, first: int, n: int) -> None:
         """Rows [first, first+n) were written into ``self.rows`` in place: compute norms and publish them."""
@@ -246,7 +261,7 @@ class VectorIndex:
         return pinned_array(shape, dtype)
 
     def search_hits(self, q: torch.Tensor, k: int, row_offset: int = 0) -> torch.Tensor:
-        """This shard's results in exchange format: uint8 CUDA tensor [nq, k, 16] = sa_hit {cosine f64, global row i64}
+        """This shard's results in exchange format: uint8 CUDA tensor [nq, k, 16] = sa_hit {score f64, global row i64}
         (``hits.view(torch.float64)[..., 0]`` / ``.view(torch.int64)[..., 1]``)."""
         assert q.is_cuda and q.dtype == torch.bfloat16 and q.dim() == 2 and q.shape[1] == self.dim
         q = q.contiguous()

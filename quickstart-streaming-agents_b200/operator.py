@@ -125,9 +125,14 @@ class VectorTable:
     def __len__(self) -> int:
         return len(self.document_id)
 
+    @property
+    def similarity(self) -> str:
+        """The index's similarity ("cosine" for an index that does not say)."""
+        return index_similarity(self.index)
+
     def upsert_many(self, document_ids, chunks, embeddings: np.ndarray, metadata=None) -> None:
         """Insert rows; a document_id seen before replaces its old row (sink-connector upsert semantics): the
-        old row's vector is zeroed, and all-zero rows are never returned by the engine."""
+        old row is tombstoned (``delete_rows``), and tombstoned rows are never returned by the engine."""
         embeddings = np.ascontiguousarray(embeddings, dtype=np.float32)
         n = len(document_ids)
         assert embeddings.shape[0] == n and len(chunks) == n
@@ -190,7 +195,8 @@ class VectorTable:
             f.flush()
             os.fsync(f.fileno())
         os.replace(tmp, os.path.join(directory, files["columns"]))
-        man = {"generation": gen, "rows": n, "files": files, "source_offsets": source_offsets or {}}
+        man = {"generation": gen, "rows": n, "files": files, "source_offsets": source_offsets or {},
+               "similarity": self.similarity}
         tmp = os.path.join(directory, "manifest.json.tmp")
         with open(tmp, "w") as f:
             json.dump(man, f)
@@ -220,7 +226,8 @@ class VectorTable:
         return cls._read_manifest(directory) is not None
 
     def load(self, directory: str) -> int:
-        """Resume from ``save``: restores the index, the side table and ``source_offsets`` (call on an empty table)."""
+        """Resume from ``save``: restores the index, the side table and ``source_offsets`` (call on an empty table).
+        A checkpoint taken under another similarity is refused (a manifest that does not name one is a cosine one)."""
         import json
         import os
         assert len(self) == 0, "load() needs an empty table"
@@ -231,6 +238,10 @@ class VectorTable:
         with open(os.path.join(directory, man["files"]["columns"]), encoding="utf-8") as f:
             for line in f:
                 rows.append(json.loads(line))
+        saved = man.get("similarity", "cosine")
+        if saved != self.similarity:
+            raise ValueError(f"checkpoint in {directory} was taken with similarity {saved!r}; this table's index uses "
+                             f"{self.similarity!r}: rankings and row terms differ, rebuild the table from the log instead")
         if len(rows) != man["rows"]:
             raise ValueError(f"snapshot mismatch: manifest says {man['rows']} rows, columns file has {len(rows)}")
         if hasattr(self.index, "restore") and "index" in man["files"]:
@@ -255,16 +266,33 @@ class VectorTable:
         self.arena_chunk.clear()
 
 
-def atlas_score(cosine: float) -> float:
-    """MongoDB Atlas reports cosine similarity normalised to [0, 1] as (1 + cos) / 2; the engine's native score is the
-    raw cosine (what BASELINE.json's numpy yardstick uses).  Apply this where a downstream consumer expects Atlas's."""
-    return 0.5 * (1.0 + cosine)
+def index_similarity(index) -> str:
+    return getattr(index, "similarity", "cosine")
+
+
+def atlas_score(score: float, similarity: str = "cosine") -> float:
+    """The score MongoDB Atlas Vector Search reports for a raw engine score, as Atlas's documentation states the
+    normalisation (restated from there, not from the reference tree): cosine and dotProduct map to [0, 1] as
+    (1 + s) / 2, euclidean distance d as 1 / (1 + d).  The engine's native score is the raw value (what BASELINE.json's
+    numpy yardstick uses).  Apply this where a downstream consumer expects Atlas's."""
+    if similarity == "euclidean":
+        return 1.0 / (1.0 + score)
+    if similarity in ("cosine", "dotProduct"):
+        return 0.5 * (1.0 + score)
+    raise ValueError(f"unknown similarity {similarity!r}")
+
+
+def wire_score_mode(score_mode: str, similarity: str) -> int:
+    """score_mode argument of sa_wire_encode_search_results: 0 raw, 1 (1 + s) / 2, 2 1 / (1 + d)."""
+    if score_mode != "atlas":
+        return 0
+    return 2 if similarity == "euclidean" else 1
 
 
 def vector_search_agg(table: VectorTable, descriptor: str, query_vectors: np.ndarray, k: int,
                       score_mode: str = "cosine") -> list[list[SearchHit]]:
     """VECTOR_SEARCH_AGG(table, DESCRIPTOR(descriptor), query_vector, k) for a batch of query vectors.
-    ``score_mode``: "cosine" (raw, default) or "atlas" ((1 + cos) / 2)."""
+    ``score_mode``: "cosine" (the raw value of the index's similarity, default) or "atlas" (``atlas_score``)."""
     if score_mode not in ("cosine", "atlas"):
         raise ValueError("score_mode must be 'cosine' or 'atlas'")
     if descriptor != table.embedding_column:
@@ -281,7 +309,7 @@ def vector_search_agg(table: VectorTable, descriptor: str, query_vectors: np.nda
         for s, i in zip(score[r].tolist(), idx[r].tolist()):
             if i < 0:
                 break
-            s = atlas_score(s) if score_mode == "atlas" else s
+            s = atlas_score(s, table.similarity) if score_mode == "atlas" else s
             hits.append(SearchHit(table.document_id[i], table.chunk[i], float(s), int(i), table.metadata[i]))
         out.append(hits)
     return out
@@ -301,7 +329,7 @@ def search_results_avro_body(table: VectorTable, query: str | None, score_row, i
             parts.append(table.avro_document_id[i])
             parts.append(table.avro_chunk[i])
             sc = float(score_row[j])
-            parts.append(b"\x02" + struct.pack("<d", atlas_score(sc) if score_mode == "atlas" else sc))
+            parts.append(b"\x02" + struct.pack("<d", atlas_score(sc, table.similarity) if score_mode == "atlas" else sc))
     return b"".join(parts)
 
 

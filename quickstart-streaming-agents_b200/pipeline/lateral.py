@@ -182,7 +182,7 @@ class LateralSearch:
                 for s, i in zip(score[r].tolist(), idx[r].tolist()):
                     if i < 0:
                         break
-                    s = atlas_score(s) if self.score_mode == "atlas" else s
+                    s = atlas_score(s, t.similarity) if self.score_mode == "atlas" else s
                     hits.append(SearchHit(t.document_id[i], t.chunk[i], float(s), int(i), t.metadata[i]))
                 header, cs, carried, names = self._enc[sid]
                 out = {c: rec.get(c) for c in carried}

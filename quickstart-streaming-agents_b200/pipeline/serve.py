@@ -35,7 +35,7 @@ import time
 import numpy as np
 
 from ..embed.stub import StubEmbedder
-from ..operator import VectorTable, rag_prompt, search_results_avro_body
+from ..operator import VectorTable, rag_prompt, search_results_avro_body, wire_score_mode
 from ..transport.filelog import Message
 from ..wire import avro, schemas
 from ..wire.registry import SchemaRegistry
@@ -102,7 +102,8 @@ class Lab2Pipeline:
         topics are files under ``log_dir``) or ``transport.kafka`` (a real cluster through confluent_kafka; ``client_conf``
         carries bootstrap.servers etc., ``log_dir`` then only holds the schema-registry stub)."""
         if score_mode not in ("cosine", "atlas"):
-            raise ValueError("score_mode must be 'cosine' (raw) or 'atlas' ((1 + cos) / 2, what MongoDB Atlas reports)")
+            raise ValueError("score_mode must be 'cosine' (the raw score of the index's similarity) or 'atlas' (what "
+                             "MongoDB Atlas reports: (1 + s) / 2, or 1 / (1 + d) for euclidean)")
         self.log_dir = log_dir
         self.table = table
         self.embedder = embedder or StubEmbedder(table.index.dim)
@@ -442,7 +443,7 @@ class Lab2Pipeline:
         args = (n, k, schemas.RESULTS_PER_QUERY, self.codec.schema_id("search_results"), text_buf.ctypes.data, toff.ctypes.data,
                 tlen.ctypes.data, score.ctypes.data, rows.ctypes.data, t.arena_document_id.data.ctypes.data,
                 t.arena_document_id.off.ctypes.data, t.arena_chunk.data.ctypes.data, t.arena_chunk.off.ctypes.data, len(t),
-                1 if self.score_mode == "atlas" else 0, int(time.time() * 1000))
+                wire_score_mode(self.score_mode, t.similarity), int(time.time() * 1000))
         lib.sa_wire_encode_search_results(*args, None, 0, rec_off.ctypes.data, C.byref(need))   # sizing pass
         out = np.empty(int(need.value), np.uint8)
         rc = lib.sa_wire_encode_search_results(*args, out.ctypes.data, out.size, rec_off.ctypes.data, C.byref(need))

@@ -2,7 +2,7 @@
 
 The path shards naturally (SURVEY.md section 8e): shard g holds the contiguous rows [offset_g, offset_g + n_g) of the
 corpus, every GPU sees the whole query block and runs the same single-GPU scan, and there is exactly ONE exchange step --
-an all-gather of each shard's packed per-query (cosine float64, global row int64) lists, k entries per query
+an all-gather of each shard's packed per-query (score float64, global row int64) lists, k entries per query
 (nq*k*16 bytes per rank: 655 KB at nq = 4096, k = 10) -- followed by a k-way merge on every rank.  No all-reduce, no
 all-to-all.
 
@@ -74,6 +74,10 @@ class ShardedIndex:
     @property
     def dim(self) -> int:
         return self.index.dim
+
+    @property
+    def similarity(self) -> str:
+        return getattr(self.index, "similarity", "cosine")
 
     # ------------------------------------------------------------------ device-resident queries
     def search(self, q: torch.Tensor, k: int):
@@ -148,7 +152,8 @@ class MultiGpuIndex:
     round-robin to the shards (SURVEY.md section 8e: "append-only streams go round-robin by epoch") and the library's
     global rows (shard * capacity + local row) are translated back through a per-shard table."""
 
-    def __init__(self, dim: int, capacity_per_gpu: int, max_batch: int, max_k: int, n_gpus: int | None = None):
+    def __init__(self, dim: int, capacity_per_gpu: int, max_batch: int, max_k: int, n_gpus: int | None = None,
+                 similarity: str = "cosine"):
         from . import capi
         from .engine import VectorIndex
         n = torch.cuda.device_count() if n_gpus is None else int(n_gpus)
@@ -156,8 +161,9 @@ class MultiGpuIndex:
             raise ValueError(f"n_gpus {n} outside [1, {torch.cuda.device_count()}]")
         self.n = n
         self.dim, self.capacity_per_gpu = dim, int(capacity_per_gpu)
-        self.shards = [VectorIndex(dim=dim, capacity=capacity_per_gpu, max_batch=max_batch, max_k=max_k, device=g)
-                       for g in range(n)]
+        self.similarity = similarity
+        self.shards = [VectorIndex(dim=dim, capacity=capacity_per_gpu, max_batch=max_batch, max_k=max_k, device=g,
+                                   similarity=similarity) for g in range(n)]
         self.lib = self.shards[0].lib
         path = capi.bundled_nccl_path()
         if path:

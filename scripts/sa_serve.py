@@ -27,7 +27,7 @@ except ImportError:
     from _local import resolve_log_dir, setup_logging
 
 
-def main(argv=None) -> int:
+def build_parser() -> argparse.ArgumentParser:
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     ap.add_argument("--log-dir", default=None)
     ap.add_argument("--dim", type=int, default=1536)
@@ -37,9 +37,13 @@ def main(argv=None) -> int:
     ap.add_argument("--gpus", type=int, default=1,
                     help="row-shard the table over this many GPUs of the box (one process, NCCL all-gather of the per-shard "
                          "candidates inside libsa_b200.so: sa_comm_create / sa_gather_merge)")
+    ap.add_argument("--similarity", default="cosine", choices=["cosine", "dotProduct", "euclidean"],
+                    help="the vector index's similarity, as in an Atlas index definition (the reference declares cosine, "
+                         "assets/pre-setup/MongoDB-Setup.md:72-83); fixed for the table and recorded in its checkpoints")
     ap.add_argument("--score-mode", default="cosine", choices=["cosine", "atlas"],
-                    help="score_i on search_results: raw cosine, or (1 + cos) / 2 as MongoDB Atlas reports it "
-                         "(the reference's index, assets/pre-setup/MongoDB-Setup.md:72-83); the ranking is the same")
+                    help="score_i on search_results: the raw score of the similarity (cosine, dot product, Euclidean "
+                         "distance), or the value MongoDB Atlas reports: (1 + s) / 2, or 1 / (1 + d) for euclidean; "
+                         "the ranking is the same")
     ap.add_argument("--lateral", action="append", default=[], choices=["lab3", "lab4"],
                     help="also run the operator joined onto an upstream stream, over the same table: lab3 = "
                          "anomalies_per_zone -> anomalies_enriched (LAB3-Walkthrough.md:225-375), lab4 = claims_to_investigate "
@@ -50,18 +54,24 @@ def main(argv=None) -> int:
     ap.add_argument("--snapshot-every", type=float, default=30.0, help="seconds between checkpoints while the table changes")
     ap.add_argument("--metrics-file", default=None, help="append one JSON line of batch-latency p50/p99 and QPS every few seconds")
     ap.add_argument("--verbose", action="store_true")
-    a = ap.parse_args(argv)
+    return ap
+
+
+def main(argv=None) -> int:
+    a = build_parser().parse_args(argv)
     setup_logging(a.verbose)
 
     from qsa_b200 import engine as engine_mod  # CUDA only; raises without a device (no CPU fallback)
     from qsa_b200.operator import VectorTable
     from qsa_b200.pipeline.serve import Lab2Pipeline
 
+    sim = {} if a.similarity == "cosine" else {"similarity": a.similarity}   # cosine is every index's default
     if a.gpus > 1:
         from qsa_b200.sharded import MultiGpuIndex
-        index = MultiGpuIndex(dim=a.dim, capacity_per_gpu=a.capacity, max_batch=a.max_batch, max_k=max(a.k, 3), n_gpus=a.gpus)
+        index = MultiGpuIndex(dim=a.dim, capacity_per_gpu=a.capacity, max_batch=a.max_batch, max_k=max(a.k, 3), n_gpus=a.gpus,
+                              **sim)
     else:
-        index = engine_mod.VectorIndex(dim=a.dim, capacity=a.capacity, max_batch=a.max_batch, max_k=max(a.k, 3))
+        index = engine_mod.VectorIndex(dim=a.dim, capacity=a.capacity, max_batch=a.max_batch, max_k=max(a.k, 3), **sim)
     table = VectorTable(index)
     if a.snapshot_dir and VectorTable.has_checkpoint(a.snapshot_dir):
         print(f"resumed {table.load(a.snapshot_dir)} rows from {a.snapshot_dir} at {table.source_offsets}", file=sys.stderr)
