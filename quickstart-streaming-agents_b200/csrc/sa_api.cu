@@ -119,7 +119,7 @@ struct sa_engine {
   float* row_term = nullptr;   // caller-owned: 1/|c| (cosine), 1 (dotProduct), |c|^2/2 (euclidean); see sa_aux.cuh
   unsigned* cmax = nullptr;    // device scalar (float bits): upper bound on |c| over the committed rows (not cosine)
   int64_t n_rows = 0;
-  CUtensorMap tmap_c[2];       // [0]: box 128 rows (cta_group 1), [1]: box 64 rows (cta_group 2, multicast)
+  CUtensorMap tmap_c[2];       // [0]: box 256 rows (cta_group 1), [1]: box 128 rows (cta_group 2, multicast)
   bool bound = false;
 
   // scratch (library-owned)
@@ -174,7 +174,7 @@ struct sa_engine {
   int opt_cta_group = 0;
   int opt_max_launch_qblocks = 0;
   int opt_max_drift = -1;  // -1 = auto (1 tile)
-  int opt_pace_gain = -1;  // -1 = auto (64 cycles/tile for CTA pairs, 32 for single CTAs), 0 = off
+  int opt_pace_gain = -1;  // -1 = auto (128 cycles/tile for CTA pairs, 64 for single CTAs), 0 = off
   int opt_pace_max = -1;   // -1 = auto (8 x gain)
   int opt_unit_map = 0;
   int opt_list_len = 0;    // 0 = auto (16 when k <= 16, else 32)
@@ -425,9 +425,10 @@ int do_search(sa_engine* e, const uint16_t* q_bf16, int nq, int k, float* out_sc
     sp.max_drift = e->opt_max_drift >= 0 ? e->opt_max_drift : 1;
     sp.pace_gain = 0;
     sp.unit_map = e->opt_unit_map;
-    // drift-control defaults: one tile of free lead, then 32 (single CTAs) or 64 (pairs) cycles of delay per K-slice
-    // issue per extra tile of lead; options "max_drift", "pace_gain" and "pace_max" override them
-    const int gain = e->opt_pace_gain >= 0 ? e->opt_pace_gain : (lp.cg == 2 ? 64 : 32);
+    // drift-control defaults: one tile of free lead, then 64 (single CTAs) or 128 (pairs) cycles of delay per K-slice
+    // issue per extra tile of lead (a tile is num_kb K slices); options "max_drift", "pace_gain" and "pace_max"
+    // override them
+    const int gain = e->opt_pace_gain >= 0 ? e->opt_pace_gain : (lp.cg == 2 ? 128 : 64);
     sp.pace_max = e->opt_pace_max >= 0 ? e->opt_pace_max : 8 * gain;
     if (lp.nqb > 1 && gain > 0) {
       sp.lane_progress = e->lane_progress + li * e->num_sms;  // this launch's slice (zero: see sa_engine)

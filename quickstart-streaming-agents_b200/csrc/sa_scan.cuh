@@ -3,7 +3,7 @@
 //  LAB4-Walkthrough.md:302-309) as one persistent, warp-specialised sm_90a kernel:
 //
 //   TMA (SWIZZLE_128B tiles of the bf16 corpus and of the query block)  ->  smem ring
-//   wgmma  Q[64 x D] . C[128 x D]^T per consumer warpgroup, fp32 accumulators in registers
+//   wgmma  Q[64 x D] . C[256 x D]^T per consumer warpgroup (two 128-row halves), fp32 accumulators in registers
 //   epilogue: accumulators -> smem -> combine with the row's term w[r] -> per-thread (thread == query) sorted register list
 //
 // The row term w[r] and the epilogue make one kernel serve every similarity of the index (sa_api.h, SA_SIM_*):
@@ -17,7 +17,8 @@
 // Work decomposition.  A "unit" is one CTA (kCG == 1, 128-query blocks) or a cluster of two CTAs (kCG == 2, 256-query
 // blocks: each CTA loads half of every corpus slice and multicasts it to both, so the pair reads each corpus tile once).
 // Unit u owns query block qb = u % nqb and tile lane tl = u / nqb and walks corpus tiles tl, tl + TL, tl + 2 TL, ...
-// (256 rows each, taken as two 128-row halves).  All units of one tile lane touch the same corpus tile at about the
+// (256 rows each: one smem stage holds a K slice of the whole tile, multiplied as two 128-row halves, so the query
+// slice crosses L2 once per tile).  All units of one tile lane touch the same corpus tile at about the
 // same time (drift control below keeps it so): it crosses HBM once and is served from L2 to the others.
 //
 // Exactness contract with the merge kernel (sa_aux.cuh).  A thread's list holds the kKL best rows of its tile lane by
@@ -34,10 +35,13 @@ namespace sa {
 
 constexpr int kBlockM = 128;  // queries per CTA
 constexpr int kBlockN = 256;  // corpus rows per tile
-constexpr int kHalfN = kWgmmaN;  // corpus rows per MMA pass: a tile is scanned as two halves
+constexpr int kHalfN = kWgmmaN;  // corpus rows per MMA: a tile is multiplied as two halves, each into its own accumulators
 constexpr int kBlockK = 64;   // bf16 per K slice = 128 B = one swizzle atom
 constexpr int kUmmaK = 16;
 constexpr int kScanThreads = 384;  // warpgroup 0: w0 TMA producer; warpgroups 1, 2: 64 queries each (MMA + epilogue)
+// Registers per thread after the roles split (setmaxnreg): 128 x 40 + 256 x 232 = 384 x 168, the launch's allocation.
+constexpr int kProducerRegs = 40;
+constexpr int kConsumerRegs = 232;
 constexpr int kChunk = 32;         // columns per list-update chunk
 constexpr int kStagingLd = kHalfN + 4;  // floats per query row of the accumulator staging buffer (conflict-free reads)
 constexpr int kWin = 16;           // tile lanes whose second-best scores an epilogue thread combines into a bound
@@ -54,10 +58,11 @@ constexpr int kEpiSub = 1;     // v = acc - w; a row is live iff w >= 0 (euclide
 
 template <int kCG>
 struct ScanCfg {
-  static constexpr int kStages = 4;
-  static constexpr int kBRows = kHalfN / kCG;  // corpus rows of a half tile loaded (and multicast) by each CTA
+  static constexpr int kStages = 3;
+  static constexpr int kBRows = kBlockN / kCG;  // corpus rows of a tile loaded (and multicast) by each CTA
   static constexpr uint32_t kABytes = kBlockM * kBlockK * 2;
-  static constexpr uint32_t kBBytes = kHalfN * kBlockK * 2;  // what lands in each CTA per stage
+  static constexpr uint32_t kBBytes = kBlockN * kBlockK * 2;  // what lands in each CTA per stage
+  static constexpr uint32_t kHalfBBytes = kHalfN * kBlockK * 2;  // the second half's rows start this far into B
   static constexpr uint32_t kStageBytes = kABytes + kBBytes;
   static constexpr uint32_t kStagingBytes = kBlockM * kStagingLd * sizeof(float);
   static constexpr uint32_t kIcBytes = 4 * kBlockN * sizeof(float);  // one 256-float scale vector per epilogue warp
@@ -72,7 +77,7 @@ struct ScanProf {
   long long prod_wait_empty;   // TMA producer blocked on a free smem slot
   long long mma_wait_full;     // first consumer warpgroup blocked on TMA data
   long long mma_wait_tempty;   // first consumer warpgroup blocked on its staging barriers (the other warps' epilogue)
-  long long epi_wait_tfull;    // first consumer warpgroup waiting for its last MMAs of a half tile to retire
+  long long epi_wait_tfull;    // first consumer warpgroup waiting for its last MMAs of a tile to retire
   long long epi_busy;          // first epilogue warp staging and scoring accumulators
   long long epi_slow_chunks;   // 32-column chunks of epilogue warp 0 that took the insertion path
   long long total;             // CTA lifetime
@@ -372,12 +377,21 @@ sa_scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const uint32_t rank = (kCG == 2) ? cluster_ctarank() : 0u;
-  const int unit = blockIdx.x / kCG;
   const int TL = p.tl_count;
   const int nqb = p.nqb;  // units per tile lane
-  const int qb = p.unit_map == 0 ? unit % nqb : unit / TL;
-  const int tl = p.unit_map == 0 ? unit / nqb : unit % TL;
-  const int walk_tiles = (p.num_tiles + p.tile_stride - 1) / p.tile_stride;  // tiles this launch visits (all lanes together)
+  // This unit's query block, tile lane and the tiles this launch visits (all lanes together).  Each role computes them
+  // after its setmaxnreg: ptxas keeps a value that is live across the register reallocation in local memory.
+  struct Walk {
+    int qb, tl, tiles;
+  };
+  auto walk_of = [&]() {
+    const int unit = blockIdx.x / kCG;
+    Walk w;
+    w.qb = p.unit_map == 0 ? unit % nqb : unit / TL;
+    w.tl = p.unit_map == 0 ? unit / nqb : unit % TL;
+    w.tiles = (p.num_tiles + p.tile_stride - 1) / p.tile_stride;
+    return w;
+  };
 
   // ------------------------------------------------------------------ one-time setup
   long long t_start = 0;
@@ -398,9 +412,12 @@ sa_scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant
   if constexpr (kCG == 2) cluster_sync_all();  // the peer's barriers are initialised before any multicast or remote arrive
 
   // ------------------------------------------------------------------ roles
-  if (warp == 0) {
-    if (lane == 0) {
+  if (warp < 4) {
+    setmaxnreg_dec<kProducerRegs>();  // the whole warpgroup: only w0's lane 0 has work
+    if (warp == 0 && lane == 0) {
       // ===== TMA producer =====
+      const Walk w = walk_of();
+      const int qb = w.qb, tl = w.tl, walk_tiles = w.tiles;
       const uint64_t c_hint = p.corpus_evict_first ? kEvictFirst : kEvictNormal;
       int stage = 0;
       uint32_t phase = 0;
@@ -425,32 +442,32 @@ sa_scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant
           for (int j = 0; j < nqb; ++j) slowest = min(slowest, ld_relaxed_gpu(pr + j));
           pace = min(max(tile_no - slowest - p.max_drift, 0) * p.pace_gain, p.pace_max);
         }
-        for (int h = 0; h < 2; ++h) {
-          for (int kb = 0; kb < p.num_kb; ++kb) {
-            if constexpr (kProf) {
-              const long long c0 = clock64();
-              mbar_wait(empty_bar(stage), phase ^ 1u);
-              waited += clock64() - c0;
-            } else {
-              mbar_wait(empty_bar(stage), phase ^ 1u);  // consumers of every CTA sharing the slot have released it
+        // one stage per K slice: the query slice and the whole tile's corpus slice (each CTA of a pair loads its
+        // kBRows rows and multicasts them to both)
+        const int c_row = t * kBlockN + static_cast<int>(rank) * Cfg::kBRows;
+        for (int kb = 0; kb < p.num_kb; ++kb) {
+          if constexpr (kProf) {
+            const long long c0 = clock64();
+            mbar_wait(empty_bar(stage), phase ^ 1u);
+            waited += clock64() - c0;
+          } else {
+            mbar_wait(empty_bar(stage), phase ^ 1u);  // consumers of every CTA sharing the slot have released it
+          }
+          if (pace > 0) {
+            const long long c0 = clock64();
+            while (clock64() - c0 < pace) {
             }
-            if (pace > 0) {
-              const long long c0 = clock64();
-              while (clock64() - c0 < pace) {
-              }
-            }
-            mbar_expect_tx(full_bar(stage), Cfg::kStageBytes);
-            tma_load_2d(a_smem(stage), &tmap_q, full_bar(stage), kb * kBlockK, q_row, kEvictLast);
-            const int c_row = t * kBlockN + h * kHalfN + static_cast<int>(rank) * Cfg::kBRows;
-            const uint32_t b_dst = b_smem(stage) + rank * (Cfg::kBRows * kBlockK * 2);
-            if constexpr (kCG == 1)
-              tma_load_2d(b_dst, &tmap_c, full_bar(stage), kb * kBlockK, c_row, c_hint);
-            else
-              tma_load_2d_multicast(b_dst, &tmap_c, full_bar(stage), kb * kBlockK, c_row, 0x3, c_hint);
-            if (++stage == kStages) {
-              stage = 0;
-              phase ^= 1u;
-            }
+          }
+          mbar_expect_tx(full_bar(stage), Cfg::kStageBytes);
+          tma_load_2d(a_smem(stage), &tmap_q, full_bar(stage), kb * kBlockK, q_row, kEvictLast);
+          const uint32_t b_dst = b_smem(stage) + rank * (Cfg::kBRows * kBlockK * 2);
+          if constexpr (kCG == 1)
+            tma_load_2d(b_dst, &tmap_c, full_bar(stage), kb * kBlockK, c_row, c_hint);
+          else
+            tma_load_2d_multicast(b_dst, &tmap_c, full_bar(stage), kb * kBlockK, c_row, 0x3, c_hint);
+          if (++stage == kStages) {
+            stage = 0;
+            phase ^= 1u;
           }
         }
         if (lockstep) st_relaxed_gpu(p.lane_progress + tl * nqb + qb, tile_no + 1);
@@ -460,10 +477,13 @@ sa_scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant
         p.prof[blockIdx.x].tiles = tile_no;
       }
     }
-  } else if (warp >= 4) {
-    // ===== consumers: warpgroup g (1 or 2) multiplies queries [64 (g-1), 64 g) of the block with each half tile, stages
-    // the accumulators in smem, and its first two warps (thread == query) feed them to the candidate lists.  The two
-    // warpgroups only meet at the smem ring's barriers. =====
+  } else {
+    // ===== consumers: warpgroup g (1 or 2) multiplies queries [64 (g-1), 64 g) of the block with each tile, one
+    // accumulator set per 128-row half, stages each half's accumulators in smem in turn, and its first two warps
+    // (thread == query) feed them to the candidate lists.  The two warpgroups only meet at the smem ring's barriers. =====
+    setmaxnreg_inc<kConsumerRegs>();  // both accumulator sets stay live through the first half's epilogue
+    const Walk w = walk_of();
+    const int qb = w.qb, tl = w.tl, walk_tiles = w.tiles;
     const int g = warp / 4 - 1;
     const int wt = threadIdx.x & 127;          // thread within the warpgroup
     const bool epi = (warp & 3) < 2;           // epilogue warp: its 32 lanes own 32 of the warpgroup's 64 queries
@@ -511,12 +531,13 @@ sa_scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant
     const size_t win_stride = static_cast<size_t>(p.nqb) * kRowsPerQb;
     unsigned* const win_q = win_on ? p.lane2 + query : nullptr;
     float pub2 = -INFINITY;   // last second-best published
-    unsigned nx2[kWin];       // the window as read at the end of the previous tile
+    unsigned nx2[kWin] = {};  // the window as read at the end of the previous tile
     bool have2 = false;
 
     const uint64_t a_desc0 = make_kmajor_sw128_desc(a_smem(0) + g * (64 * kBlockK * 2));
     const uint64_t b_desc0 = make_kmajor_sw128_desc(b_smem(0));
     constexpr uint64_t kStageDesc = Cfg::kStageBytes >> 4;  // one stage further in the descriptors' address field
+    constexpr uint64_t kHalfBDesc = Cfg::kHalfBBytes >> 4;  // the tile's second half in B
     int stage = 0;
     uint32_t phase = 0;
     long long w_full = 0, w_stage = 0, w_mma = 0, busy = 0, slow_chunks = 0;
@@ -540,61 +561,73 @@ sa_scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant
         float4* dst = reinterpret_cast<float4*>(ic + 8 * lane);
         dst[0] = make_float4(sc(nx0.x), sc(nx0.y), sc(nx0.z), sc(nx0.w));
         dst[1] = make_float4(sc(nx1.x), sc(nx1.y), sc(nx1.z), sc(nx1.w));
-        if (ti + TL < walk_tiles) fetch_ic((ti + TL) * p.tile_stride);  // prefetch the next tile's inverse norms
-        __syncwarp();                                                     // ic[] visible to the whole warp
+        __syncwarp();  // ic[] visible to the whole warp
       }
+      // The window is consumed.  Cleared on every path, it holds no value across the MMAs: the compiler cannot tell
+      // that `have2` is false until the next fetch, and would otherwise keep kWin registers live through the tile.
+#pragma unroll
+      for (int i = 0; i < kWin; ++i) nx2[i] = 0u;
       float* dbg_row = nullptr;
       if constexpr (kMode == kModeDots) {
         if (own_query && p.dbg_dots != nullptr && t == p.dbg_tile) dbg_row = p.dbg_dots + static_cast<size_t>(query) * kBlockN;
       }
-      for (int h = 0; h < 2; ++h) {
-        // ---- MMA: acc = Q[64 x D] . C[half tile]^T, K slice by K slice; a slot is released once the MMAs reading it
-        // have retired (wait_group 1 after the next slice's issue keeps one slice in flight)
-        float acc[64];  // dead between halves: the first MMA of a half overwrites it
-        int prev_stage = -1;
-        for (int kb = 0; kb < p.num_kb; ++kb) {
-          if constexpr (kProf) {
-            const long long c0 = clock64();
-            mbar_wait(full_bar(stage), phase, static_cast<uint32_t>(p.wait_hint_ns));
-            w_full += clock64() - c0;
-          } else {
-            mbar_wait(full_bar(stage), phase, static_cast<uint32_t>(p.wait_hint_ns));
-          }
-          wgmma_fence();
-          wgmma_fence_operands(acc);
+      // ---- MMA: acc0 = Q[64 x D] . C[rows 0..127 of the tile]^T, acc1 the same for rows 128..255, K slice by K slice,
+      // both from the same A slice; a slot is released once the MMAs reading it have retired (wait_group 1 after the
+      // next slice's issue keeps one slice in flight)
+      float acc0[64], acc1[64];  // dead between tiles: the first MMA of a tile overwrites them
+      int prev_stage = -1;
+      for (int kb = 0; kb < p.num_kb; ++kb) {
+        if constexpr (kProf) {
+          const long long c0 = clock64();
+          mbar_wait(full_bar(stage), phase, static_cast<uint32_t>(p.wait_hint_ns));
+          w_full += clock64() - c0;
+        } else {
+          mbar_wait(full_bar(stage), phase, static_cast<uint32_t>(p.wait_hint_ns));
+        }
+        wgmma_fence();
+        wgmma_fence_operands(acc0);
+        wgmma_fence_operands(acc1);
 #pragma unroll
-          for (int k = 0; k < kBlockK / kUmmaK; ++k) {
-            // +32 B along K inside the 128-B swizzle atom = +2 in the (addr >> 4) field
-            wgmma_m64n128k16_bf16(acc, a_desc0 + stage * kStageDesc + 2u * k, b_desc0 + stage * kStageDesc + 2u * k,
-                                  (kb | k) != 0 ? 1u : 0u);
-          }
-          wgmma_commit();
-          wgmma_fence_operands(acc);
-          if (prev_stage >= 0) {
-            wgmma_wait<1>();
-            if (signaller) {
-              mbar_arrive(empty_bar(prev_stage));
-              if constexpr (kCG == 2) mbar_arrive_cluster(empty_bar(prev_stage), rank ^ 1u);
-            }
-          }
-          prev_stage = stage;
-          if (++stage == kStages) {
-            stage = 0;
-            phase ^= 1u;
+        for (int k = 0; k < kBlockK / kUmmaK; ++k) {
+          // +32 B along K inside the 128-B swizzle atom = +2 in the (addr >> 4) field
+          const uint64_t a_desc = a_desc0 + stage * kStageDesc + 2u * k;
+          const uint64_t b_desc = b_desc0 + stage * kStageDesc + 2u * k;
+          wgmma_m64n128k16_bf16(acc0, a_desc, b_desc, (kb | k) != 0 ? 1u : 0u);
+          wgmma_m64n128k16_bf16(acc1, a_desc, b_desc + kHalfBDesc, (kb | k) != 0 ? 1u : 0u);
+        }
+        wgmma_commit();
+        wgmma_fence_operands(acc0);
+        wgmma_fence_operands(acc1);
+        if (prev_stage >= 0) {
+          wgmma_wait<1>();
+          if (signaller) {
+            mbar_arrive(empty_bar(prev_stage));
+            if constexpr (kCG == 2) mbar_arrive_cluster(empty_bar(prev_stage), rank ^ 1u);
           }
         }
-        long long c0 = 0;
-        if constexpr (kProf) c0 = clock64();
-        wgmma_wait<0>();
-        wgmma_fence_operands(acc);
-        if (signaller) {
-          mbar_arrive(empty_bar(prev_stage));
-          if constexpr (kCG == 2) mbar_arrive_cluster(empty_bar(prev_stage), rank ^ 1u);
+        prev_stage = stage;
+        if (++stage == kStages) {
+          stage = 0;
+          phase ^= 1u;
         }
+      }
+      long long c0 = 0;
+      if constexpr (kProf) c0 = clock64();
+      wgmma_wait<0>();
+      wgmma_fence_operands(acc0);
+      wgmma_fence_operands(acc1);
+      if (signaller) {
+        mbar_arrive(empty_bar(prev_stage));
+        if constexpr (kCG == 2) mbar_arrive_cluster(empty_bar(prev_stage), rank ^ 1u);
+      }
+      if constexpr (kProf) w_mma += clock64() - c0;
+      // prefetch the next tile's row terms: issued after the MMAs, so that they hold no registers across them
+      if (epi && ti + TL < walk_tiles) fetch_ic((ti + TL) * p.tile_stride);
+      // ---- one half at a time through the staging buffer, rows in ascending order
+      auto stage_and_score = [&](const float (&acc)[64], int h) {
         long long c1 = 0;
         if constexpr (kProf) c1 = clock64();
-        // ---- stage the accumulators: the previous half's readers are done with the buffer first
-        named_bar_sync(named_bar, 128);
+        named_bar_sync(named_bar, 128);  // the previous half's readers are done with the buffer
 #pragma unroll
         for (int j = 0; j < 16; ++j) {
           const int r = 16 * (wt >> 5) + ((wt & 31) >> 2);
@@ -607,13 +640,14 @@ sa_scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant
         if constexpr (kProf) c2 = clock64();
         if (epi)
           slow += epilogue_half<kKL, kMode, kEpi>(L, stg + wt * kStagingLd, ic + h * kHalfN, t * kBlockN + h * kHalfN,
-                                            dbg_row != nullptr ? dbg_row + h * kHalfN : nullptr);
+                                                  dbg_row != nullptr ? dbg_row + h * kHalfN : nullptr);
         if constexpr (kProf) {
-          w_mma += c1 - c0;
           w_stage += c2 - c1;
           busy += clock64() - c2;
         }
-      }
+      };
+      stage_and_score(acc0, 0);
+      stage_and_score(acc1, 1);
       if constexpr (kProf) slow_chunks += slow;
       if (epi) {
         if (L.slot != nullptr) {
@@ -633,11 +667,15 @@ sa_scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant
               st_relaxed_gpu_u32(win_q + static_cast<size_t>(tl) * win_stride, float_to_key(pub2));
             }
             if (fetch && ti + TL < walk_tiles) {
+              // the stride goes through an opaque move so that the kWin addresses are formed here, at each fetch:
+              // hoisted out of the tile loop they would hold 2 kWin registers across the MMAs, and spill
+              size_t stride = win_stride;
+              asm volatile("" : "+l"(stride));
 #pragma unroll
               for (int i = 0; i < kWin; ++i) {
                 int ln = tl + i;
                 ln -= (ln >= TL) ? TL : 0;
-                nx2[i] = ld_relaxed_gpu_u32(win_q + static_cast<size_t>(ln) * win_stride);
+                nx2[i] = ld_relaxed_gpu_u32(win_q + static_cast<size_t>(ln) * stride);
               }
               have2 = true;
             }

@@ -85,6 +85,18 @@ __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
+// Per-thread register budget of the executing warpgroup (every warp of the warpgroup executes the same one).  dec hands
+// registers back to the CTA's pool, inc blocks until the pool has them; ptxas allocates the code that follows within
+// the new budget.
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
+}
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N));
+}
+
 // ----------------------------------------------------------------------------------------------
 // gpu-scope flags in global memory
 // ----------------------------------------------------------------------------------------------

@@ -4,7 +4,9 @@ counters for each warp role) and the production build (CUDA-event time) on the B
 
     prod   : scan ms (mean of --iters back-to-back searches after a preheat), achieved GB/s and TFLOP/s
     roles  : cycles per tile -- TMA producer blocked on a free smem slot, MMA issuer blocked on data / on the epilogue,
-             epilogue blocked on the MMA / busy, share of 32-column chunks that took the insertion path
+             epilogue blocked on the MMA / busy, share of 32-column chunks that took the insertion path.  The MMAs of
+             both halves of a tile retire together, so "blocked on the MMA" is one wait per tile; staging and epilogue
+             are summed over the tile's two halves.
 
 A role that is never blocked is the bottleneck.  Usage (GPU box):  python tools/gpu_prof.py [--shapes cfg5,b128,...]
 """
