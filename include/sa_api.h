@@ -78,6 +78,25 @@ void sa_engine_destroy(sa_engine* e);
  * rows' norms that the search's certificate uses is recomputed over them. */
 int sa_corpus_bind(sa_engine* e, void* rows_bf16_dev, float* row_term_dev, int64_t n_valid);
 
+/* --- pre-filtered search (the "filter" of Atlas's $vectorSearch over an index's {"type": "filter"} fields) ----------
+ * Row tags: one caller-owned 64-bit word per row, a device array of [capacity_rows] entries, 16-byte aligned.  A set bit
+ * means "this row carries value v of filter field f"; which bit stands for which (field, value) is the caller's mapping
+ * (the Python layer's FilterSchema).  Tags of rows at or past the committed row count are never read.  The caller
+ * writes a new row's tag before it appends or commits the row, exactly as with the row itself; tags of committed rows
+ * may be rewritten between searches.  row_tags_dev == NULL detaches the array. */
+int sa_corpus_bind_tags(sa_engine* e, uint64_t* row_tags_dev);
+
+/* The per-query predicate in one fixed normal form.  Row r is eligible for query i iff it is live (as for an unfiltered
+ * search) and pass(tags[r], filters[i]):
+ *   (t & all_of) == all_of  and  (t & none_of) == 0  and  for each j: any_of[j] == 0 or (t & any_of[j]) != 0
+ * All zero matches every row.  The search's answer is then exactly the unfiltered definition over the eligible rows
+ * (fewer than k eligible rows: the remaining slots are empty). */
+typedef struct sa_filter {
+  uint64_t all_of;    /* every bit must be set on the row */
+  uint64_t none_of;   /* no bit may be set */
+  uint64_t any_of[2]; /* each nonzero word: at least one of its bits must be set; 0 = no constraint */
+} sa_filter;          /* all zero = matches every row */
+
 /* --- ingest (the "documents -> documents_embed -> MongoDB sink" half of Lab2, LAB2-Walkthrough.md:41-51,
  *     fed by scripts/publish_docs.py:225-351; embeddings arrive as ARRAY<FLOAT>, main.tf:141,215) ------- */
 /* Rows [first_row, first_row+n_new) were written in place as bf16 by the caller: compute their row terms and
@@ -116,6 +135,19 @@ int sa_search_host(sa_engine* e, const float* q_f32_host, int nq, int k, float* 
 int sa_search_host_submit(sa_engine* e, int slot, const float* q_f32_host, int nq, int k);
 int sa_search_host_wait(sa_engine* e, int slot, float* out_score_host, int32_t* out_idx_host);
 
+/* Filtered twins of the searches above: `filters` holds nq sa_filter entries, device memory for the device forms and
+ * host memory for the host forms.  They fail with SA_ERR_ARG when filters is NULL or the engine has no tags bound
+ * (sa_corpus_bind_tags).  The host forms stage the filters in the slot's own pinned and device buffers, so the caller
+ * may reuse its filter array as soon as the call returns; sa_search_host_wait collects a filtered submit as well. */
+int sa_search_filtered(sa_engine* e, const void* q_bf16_dev, const sa_filter* filters_dev, int nq, int k,
+                       float* out_score_dev, int32_t* out_idx_dev, double* out_score64_dev, uintptr_t stream);
+int sa_search_f32_filtered(sa_engine* e, const float* q_f32_dev, const sa_filter* filters_dev, int nq, int k,
+                           float* out_score_dev, int32_t* out_idx_dev, double* out_score64_dev, uintptr_t stream);
+int sa_search_host_filtered(sa_engine* e, const float* q_f32_host, const sa_filter* filters_host, int nq, int k,
+                            float* out_score_host, int32_t* out_idx_host);
+int sa_search_host_submit_filtered(sa_engine* e, int slot, const float* q_f32_host, const sa_filter* filters_host, int nq,
+                                   int k);
+
 /* --- multi-GPU (SURVEY.md section 8e): the corpus is row-sharded, every GPU searches its shard with the same single-GPU
  *     path, the per-shard results cross NVLink in ONE all-gather of packed (cosine f64, global row) lists -- nq*k*16 bytes
  *     per rank -- and every rank merges them to the global top-k by (cosine desc, global row asc).  This is the whole of
@@ -128,6 +160,9 @@ typedef struct sa_hit {
 /* This shard's results in exchange format (device buffer [nq x k]), e.g. for a caller-run collective. */
 int sa_search_hits(sa_engine* e, const void* q_bf16_dev, int nq, int k, int64_t row_offset, sa_hit* out_hits_dev,
                    uintptr_t stream);
+/* Filtered twin (filters_dev: [nq] on the device); each shard filters by its own tags. */
+int sa_search_hits_filtered(sa_engine* e, const void* q_bf16_dev, const sa_filter* filters_dev, int nq, int k,
+                            int64_t row_offset, sa_hit* out_hits_dev, uintptr_t stream);
 /* Merge gathered hit lists [n_shards x nq x k] into the global top-k: out_score [nq x k] fp32, out_row [nq x k] int64.
  * The order is that of e's similarity (ascending for distances). */
 int sa_merge_hits(sa_engine* e, const sa_hit* hits_dev, int n_shards, int nq, int k, float* out_score_dev,
@@ -160,6 +195,11 @@ int sa_sharded_search(sa_comm* c, sa_engine* e, const void* q_bf16_dev, int nq, 
 int sa_sharded_search_host_submit(sa_comm* c, sa_engine* e, int slot, const float* q_f32_host, int nq, int k,
                                   int64_t row_offset);
 int sa_sharded_search_host_wait(sa_comm* c, sa_engine* e, int slot, float* out_score_host, int64_t* out_row_host);
+/* Filtered twins: every rank passes the same filters; each filters its shard by its own tags. */
+int sa_sharded_search_filtered(sa_comm* c, sa_engine* e, const void* q_bf16_dev, const sa_filter* filters_dev, int nq,
+                               int k, int64_t row_offset, float* out_score_dev, int64_t* out_row_dev, uintptr_t stream);
+int sa_sharded_search_host_submit_filtered(sa_comm* c, sa_engine* e, int slot, const float* q_f32_host,
+                                           const sa_filter* filters_host, int nq, int k, int64_t row_offset);
 
 /* Single process, all GPUs of the communicator: host fp32 queries in, merged host results out.  engines[g] lives on the
  * communicator's device g and holds the shard whose first global row is shard_offsets[g].  sa_gather_merge blocks;
@@ -169,6 +209,11 @@ int sa_gather_merge(sa_comm* c, sa_engine* const* engines, const float* q_f32_ho
 int sa_gather_merge_submit(sa_comm* c, sa_engine* const* engines, int slot, const float* q_f32_host, int nq, int k,
                            const int64_t* shard_offsets);
 int sa_gather_merge_wait(sa_comm* c, sa_engine* const* engines, int slot, float* out_score_host, int64_t* out_row_host);
+/* Filtered twins (filters_host: [nq] host sa_filter, the same for every shard; every engine needs its tags bound). */
+int sa_gather_merge_filtered(sa_comm* c, sa_engine* const* engines, const float* q_f32_host, const sa_filter* filters_host,
+                             int nq, int k, const int64_t* shard_offsets, float* out_score_host, int64_t* out_row_host);
+int sa_gather_merge_submit_filtered(sa_comm* c, sa_engine* const* engines, int slot, const float* q_f32_host,
+                                    const sa_filter* filters_host, int nq, int k, const int64_t* shard_offsets);
 
 /* --- observability ------------------------------------------------------------------------------------
  * CUDA-event times of the most recent search on this engine (synchronises on its last event):
@@ -195,7 +240,8 @@ int sa_timing_mean(sa_engine* e, int n, float* scan_ms_mean, float* total_ms_mea
 int sa_set_option(sa_engine* e, const char* name, int64_t value);
 /* "num_sms", "dim", "capacity", "n_rows", "max_batch", "max_k", "last_grid", "last_fix_entries" (with "count_fix"),
  * "eps_rel_e12" (the certificate's relative error bound, times 1e12), "similarity" (SA_SIM_*), "cmax_bits" (fp32 bits of
- * the device-side upper bound on the committed rows' norms; dotProduct and euclidean only, 0 for cosine; synchronous). */
+ * the device-side upper bound on the committed rows' norms; dotProduct and euclidean only, 0 for cosine; synchronous),
+ * "has_tags" (1 when a row tag array is bound, sa_corpus_bind_tags). */
 int sa_get_info(const sa_engine* e, const char* name, int64_t* value);
 /* Per-CTA profile records of the last scan launch run with "profile" = 1 (synchronises the device): out_host receives
  * n_ctas x 8 int64 {TMA producer wait for a free slot, MMA issuer wait for data, MMA issuer wait for the epilogue,
@@ -226,6 +272,8 @@ int sa_debug_list_insert(const float* score, const int32_t* row, int n, int list
  * one query as order-preserving keys, 0 = not published yet) the (list_len/2)-th largest key (0 = no bound yet);
  * out_sorted (optional) receives each window sorted descending by the kernel's 16-input network. */
 int sa_debug_window_bound(const uint32_t* keys, int n_windows, int list_len, uint32_t* out_bound, uint32_t* out_sorted);
+/* The filter predicate (sa_filter) exactly as the scan and the fallback scan evaluate it: out[i] = pass(tags[i], *f). */
+int sa_debug_filter_pass(const uint64_t* tags, int n, const sa_filter* f, uint8_t* out);
 
 /* Pinned host memory for callers that want truly asynchronous staging. */
 int sa_host_alloc(void** out, uint64_t bytes);

@@ -44,6 +44,11 @@ EXPORTS = (
     "sa_last_timing", "sa_timing_mean", "sa_set_option",
     "sa_get_info", "sa_scan_profile", "sa_debug_tile_dots", "sa_debug_plan", "sa_debug_float_keys", "sa_debug_bf16_round",
     "sa_debug_merge_keys", "sa_debug_list_insert", "sa_debug_window_bound", "sa_host_alloc", "sa_host_free",
+    # pre-filtered search
+    "sa_corpus_bind_tags", "sa_search_filtered", "sa_search_f32_filtered", "sa_search_host_filtered",
+    "sa_search_host_submit_filtered", "sa_search_hits_filtered", "sa_sharded_search_filtered",
+    "sa_sharded_search_host_submit_filtered", "sa_gather_merge_filtered", "sa_gather_merge_submit_filtered",
+    "sa_debug_filter_pass",
     # include/sa_wire.h
     "sa_wire_split_log", "sa_wire_decode_queries_embed", "sa_wire_decode_documents_embed", "sa_wire_encode_search_results", "sa_wire_encode_queries_embed",
 )
@@ -126,6 +131,17 @@ def load() -> C.CDLL:
         "sa_wire_encode_search_results": (i32, [i32, i32, i32, C.c_uint32, vp, vp, vp, vp, vp, vp, vp, vp, vp, i64, i32, i64,
                                                 vp, u64, vp, C.POINTER(u64)]),
         "sa_wire_encode_queries_embed": (i32, [i32, i32, C.c_uint32, vp, vp, vp, vp, i64, vp, u64, vp, C.POINTER(u64)]),
+        "sa_corpus_bind_tags": (i32, [vp, vp]),
+        "sa_search_filtered": (i32, [vp, vp, vp, i32, i32, vp, vp, vp, vp]),
+        "sa_search_f32_filtered": (i32, [vp, vp, vp, i32, i32, vp, vp, vp, vp]),
+        "sa_search_host_filtered": (i32, [vp, vp, vp, i32, i32, vp, vp]),
+        "sa_search_host_submit_filtered": (i32, [vp, i32, vp, vp, i32, i32]),
+        "sa_search_hits_filtered": (i32, [vp, vp, vp, i32, i32, i64, vp, vp]),
+        "sa_sharded_search_filtered": (i32, [vp, vp, vp, vp, i32, i32, i64, vp, vp, vp]),
+        "sa_sharded_search_host_submit_filtered": (i32, [vp, vp, i32, vp, vp, i32, i32, i64]),
+        "sa_gather_merge_filtered": (i32, [vp, C.POINTER(vp), vp, vp, i32, i32, C.POINTER(i64), vp, vp]),
+        "sa_gather_merge_submit_filtered": (i32, [vp, C.POINTER(vp), i32, vp, vp, i32, i32, C.POINTER(i64)]),
+        "sa_debug_filter_pass": (i32, [vp, i32, vp, vp]),
         "sa_host_alloc": (i32, [C.POINTER(vp), u64]),
         "sa_host_free": (i32, [vp]),
     }

@@ -12,6 +12,7 @@
 
 #include <algorithm>
 #include <cstdarg>
+#include <cstddef>
 #include <cstdio>
 #include <cstring>
 #include <string>
@@ -118,6 +119,7 @@ struct sa_engine {
   uint16_t* corpus = nullptr;  // caller-owned
   float* row_term = nullptr;   // caller-owned: 1/|c| (cosine), 1 (dotProduct), |c|^2/2 (euclidean); see sa_aux.cuh
   unsigned* cmax = nullptr;    // device scalar (float bits): upper bound on |c| over the committed rows (not cosine)
+  unsigned long long* row_tags = nullptr;  // caller-owned [capacity] filter tags (sa_corpus_bind_tags), or nullptr
   int64_t n_rows = 0;
   CUtensorMap tmap_c[2];       // [0]: box 256 rows (cta_group 1), [1]: box 128 rows (cta_group 2, multicast)
   bool bound = false;
@@ -143,6 +145,8 @@ struct sa_engine {
     float* h_score = nullptr;  // pinned [max_batch][max_k]
     int* h_idx = nullptr;      // pinned
     long long* h_row64 = nullptr;  // pinned [max_batch][max_k] (sharded searches return global rows)
+    sa::Filter* h_f = nullptr;     // pinned [max_batch] filters of a filtered search ...
+    sa::Filter* d_f = nullptr;     // ... and their device copy
     bool sharded = false;
     cudaEvent_t done = nullptr;
     int nq = 0, k = 0;
@@ -274,12 +278,13 @@ std::vector<LaunchPlan> plan_search(int num_sms, int max_launch_qblocks, int nq,
 template <int kCG, int kKL, int kMode, int kEpi = sa::kEpiMul>
 int launch_scan(const CUtensorMap& tq, const CUtensorMap& tc, const sa::ScanParams& p, int grid, cudaStream_t st) {
   auto kern = sa::sa_scan_kernel<kCG, kKL, kMode, kEpi>;
+  constexpr uint32_t kSmem = sa::ScanCfg<kCG, (kEpi & sa::kEpiFilt) != 0>::kSmemBytes;
   // per-device attribute; a few microseconds, so set it on every launch rather than caching per device
-  SA_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, sa::ScanCfg<kCG>::kSmemBytes));
+  SA_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem));
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(grid);
   cfg.blockDim = dim3(sa::kScanThreads);
-  cfg.dynamicSmemBytes = sa::ScanCfg<kCG>::kSmemBytes;
+  cfg.dynamicSmemBytes = kSmem;
   cfg.stream = st;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeClusterDimension;
@@ -292,10 +297,25 @@ int launch_scan(const CUtensorMap& tq, const CUtensorMap& tc, const sa::ScanPara
   return SA_OK;
 }
 
-// epi: sa::kEpiMul (cosine, dotProduct) or sa::kEpiSub (euclidean).  The debug dump reads raw accumulators, which do
-// not depend on the epilogue, so it has the multiply form only.
+// epi: sa::kEpiMul (cosine, dotProduct) or sa::kEpiSub (euclidean), | sa::kEpiFilt for a filtered search.  The debug
+// dump reads raw accumulators, which do not depend on the epilogue, so it has the multiply form only; the filtered scan
+// has the production build only.
 int launch_scan_dispatch(int cg, int kl, int mode, int epi, const CUtensorMap& tq, const CUtensorMap& tc,
                          const sa::ScanParams& p, int grid, cudaStream_t st) {
+  if (epi & sa::kEpiFilt) {
+    if (mode != sa::kModeProd) return fail(SA_ERR_ARG, "a filtered search has no profiling or debug build of the scan");
+    constexpr int kM = sa::kEpiMul | sa::kEpiFilt, kS = sa::kEpiSub | sa::kEpiFilt;
+    const bool sub = (epi & 1) == sa::kEpiSub;
+    if (cg == 1 && kl == 16) return sub ? launch_scan<1, 16, sa::kModeProd, kS>(tq, tc, p, grid, st)
+                                        : launch_scan<1, 16, sa::kModeProd, kM>(tq, tc, p, grid, st);
+    if (cg == 1 && kl == 32) return sub ? launch_scan<1, 32, sa::kModeProd, kS>(tq, tc, p, grid, st)
+                                        : launch_scan<1, 32, sa::kModeProd, kM>(tq, tc, p, grid, st);
+    if (cg == 2 && kl == 16) return sub ? launch_scan<2, 16, sa::kModeProd, kS>(tq, tc, p, grid, st)
+                                        : launch_scan<2, 16, sa::kModeProd, kM>(tq, tc, p, grid, st);
+    if (cg == 2 && kl == 32) return sub ? launch_scan<2, 32, sa::kModeProd, kS>(tq, tc, p, grid, st)
+                                        : launch_scan<2, 32, sa::kModeProd, kM>(tq, tc, p, grid, st);
+    return fail(SA_ERR_ARG, "no scan instantiation for cta_group %d list %d", cg, kl);
+  }
   if (epi == sa::kEpiSub) {
     if (mode == sa::kModeProf) {
       if (cg == 1 && kl == 16) return launch_scan<1, 16, sa::kModeProf, sa::kEpiSub>(tq, tc, p, grid, st);
@@ -362,10 +382,19 @@ int zero_scan_scratch(sa_engine* e, cudaStream_t st) {
   return SA_OK;
 }
 
+// A filtered search needs its filters and a bound tag array.
+int check_filtered(const sa_engine* e, const void* filters) {
+  if (!filters) return fail(SA_ERR_ARG, "null filters");
+  if (!e->row_tags) return fail(SA_ERR_ARG, "filtered search without row tags (call sa_corpus_bind_tags)");
+  return SA_OK;
+}
+
 // One search = per scan launch {scan kernel, merge/certify kernel}, then one fixup kernel (exact fallback scan of the
 // ambiguous (query, lane) pairs -- normally none -- and conversion of the internal result to the caller's arrays).
+// filters (device, [nq]) != nullptr: a filtered search; every kernel sees only the rows that pass each query's filter.
 int do_search(sa_engine* e, const uint16_t* q_bf16, int nq, int k, float* out_score, int32_t* out_idx,
-              double* out_score64, sa::PackedHit* out_packed, int64_t row_offset, cudaStream_t st) {
+              double* out_score64, sa::PackedHit* out_packed, int64_t row_offset, cudaStream_t st,
+              const sa::Filter* filters = nullptr) {
   if (nq <= 0 || nq > e->max_batch) return fail(SA_ERR_CAPACITY, "nq %d outside [1, max_batch %d]", nq, e->max_batch);
   if (k <= 0 || k > e->max_k) return fail(SA_ERR_ARG, "k %d outside [1, max_k %d]", k, e->max_k);
   if (!q_bf16 || !out_score || !out_idx) return fail(SA_ERR_ARG, "null buffer");
@@ -383,7 +412,7 @@ int do_search(sa_engine* e, const uint16_t* q_bf16, int nq, int k, float* out_sc
   if (static_cast<int>(plan.size()) > kMaxLaunches)
     return fail(SA_ERR_CAPACITY, "batch needs %zu scan launches (max %d)", plan.size(), kMaxLaunches);
   const int mode = e->opt_profile ? sa::kModeProf : sa::kModeProd;
-  const int epi = e->sim == SA_SIM_EUCLIDEAN ? sa::kEpiSub : sa::kEpiMul;
+  const int epi = (e->sim == SA_SIM_EUCLIDEAN ? sa::kEpiSub : sa::kEpiMul) | (filters != nullptr ? sa::kEpiFilt : 0);
   const float eps_rel = scan_eps_rel(e->dim);
 
   // The candidate lists, shared thresholds and drift counters are one set of scratch buffers: a search issued on
@@ -445,6 +474,10 @@ int do_search(sa_engine* e, const uint16_t* q_bf16, int nq, int k, float* out_sc
     sp.dbg_tile = -1;
     sp.dbg_times = e->opt_record_times ? e->dbg_times : nullptr;
     sp.prof = e->prof;
+    if (filters != nullptr) {
+      sp.row_tags = e->row_tags;
+      sp.filters = filters + lp.q0;
+    }
     const int grid = lp.nqb * lp.tl * lp.cg;
     e->last_grid = grid;
     min_tl = std::min(min_tl, lp.tl);
@@ -555,6 +588,8 @@ int do_search(sa_engine* e, const uint16_t* q_bf16, int nq, int k, float* out_sc
     fp.zero_b_n = static_cast<int>(plan.size()) * e->num_sms;
     fp.zero_c = e->lane2;
     fp.zero_c_n = e->opt_window_bound ? static_cast<int>(plan.size()) * e->num_sms * 128 : 0;
+    fp.row_tags = filters != nullptr ? e->row_tags : nullptr;
+    fp.filters = filters;
     const size_t smem = static_cast<size_t>(e->dim) * sizeof(float);
     if (smem > 48 * 1024)
       SA_CUDA(cudaFuncSetAttribute(sa::sa_fixup_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
@@ -605,6 +640,11 @@ void run_list(const float* score, const int32_t* row, int n, const float* floor_
 }  // namespace
 
 extern "C" {
+
+static_assert(sizeof(sa_filter) == sizeof(sa::Filter) && offsetof(sa_filter, all_of) == offsetof(sa::Filter, all_of) &&
+                  offsetof(sa_filter, none_of) == offsetof(sa::Filter, none_of) &&
+                  offsetof(sa_filter, any_of) == offsetof(sa::Filter, any_of),
+              "sa_filter and sa::Filter must share one layout");
 
 int sa_version(void) { return 100; }
 
@@ -693,6 +733,8 @@ int sa_engine_create_sim(sa_engine** out, int device, int dim, int64_t capacity_
     SA_TRY(cudaHostAlloc(&e->slot[i].h_score, relems * 4, cudaHostAllocDefault));
     SA_TRY(cudaHostAlloc(&e->slot[i].h_idx, relems * 4, cudaHostAllocDefault));
     SA_TRY(cudaHostAlloc(&e->slot[i].h_row64, relems * sizeof(long long), cudaHostAllocDefault));
+    SA_TRY(cudaHostAlloc(&e->slot[i].h_f, static_cast<size_t>(max_batch) * sizeof(sa::Filter), cudaHostAllocDefault));
+    SA_TRY(cudaMalloc(&e->slot[i].d_f, static_cast<size_t>(max_batch) * sizeof(sa::Filter)));
     SA_TRY(cudaEventCreateWithFlags(&e->slot[i].done, cudaEventDisableTiming));
   }
   SA_TRY(cudaHostAlloc(&e->h_stage, static_cast<size_t>(e->stage_rows) * dim * 4, cudaHostAllocDefault));
@@ -750,6 +792,8 @@ void sa_engine_destroy(sa_engine* e) {
     cudaFreeHost(e->slot[i].h_score);
     cudaFreeHost(e->slot[i].h_idx);
     cudaFreeHost(e->slot[i].h_row64);
+    cudaFreeHost(e->slot[i].h_f);
+    cudaFree(e->slot[i].d_f);
     if (e->slot[i].done) cudaEventDestroy(e->slot[i].done);
   }
   cudaFreeHost(e->h_stage);
@@ -799,6 +843,13 @@ int sa_corpus_bind(sa_engine* e, void* rows_bf16_dev, float* row_term_dev, int64
       SA_CUDA(cudaGetLastError());
     }
   }
+  return SA_OK;
+}
+
+int sa_corpus_bind_tags(sa_engine* e, uint64_t* row_tags_dev) {
+  if (!e) return fail(SA_ERR_ARG, "null engine");
+  if (reinterpret_cast<uintptr_t>(row_tags_dev) % 16) return fail(SA_ERR_ARG, "row tags must be 16-byte aligned");
+  e->row_tags = reinterpret_cast<unsigned long long*>(row_tags_dev);
   return SA_OK;
 }
 
@@ -889,8 +940,18 @@ int sa_search(sa_engine* e, const void* q_bf16_dev, int nq, int k, float* out_sc
                    nullptr, 0, reinterpret_cast<cudaStream_t>(stream));
 }
 
-int sa_search_f32(sa_engine* e, const float* q_f32_dev, int nq, int k, float* out_score_dev, int32_t* out_idx_dev,
-                  double* out_score64_dev, uintptr_t stream) {
+int sa_search_filtered(sa_engine* e, const void* q_bf16_dev, const sa_filter* filters_dev, int nq, int k,
+                       float* out_score_dev, int32_t* out_idx_dev, double* out_score64_dev, uintptr_t stream) {
+  int rc = check_engine(e);
+  if (rc) return rc;
+  rc = check_filtered(e, filters_dev);
+  if (rc) return rc;
+  return do_search(e, static_cast<const uint16_t*>(q_bf16_dev), nq, k, out_score_dev, out_idx_dev, out_score64_dev,
+                   nullptr, 0, reinterpret_cast<cudaStream_t>(stream), reinterpret_cast<const sa::Filter*>(filters_dev));
+}
+
+static int search_f32(sa_engine* e, const float* q_f32_dev, const sa::Filter* filters, int nq, int k,
+                      float* out_score_dev, int32_t* out_idx_dev, double* out_score64_dev, uintptr_t stream) {
   int rc = check_engine(e);
   if (rc) return rc;
   if (!q_f32_dev) return fail(SA_ERR_ARG, "null queries");
@@ -902,9 +963,24 @@ int sa_search_f32(sa_engine* e, const float* q_f32_dev, int nq, int k, float* ou
   sa::sa_convert_rows_kernel<<<static_cast<unsigned>((threads + 255) / 256), 256, 0, st>>>(q_f32_dev, e->q_bf16,
                                                                                          nullptr, nq, e->dim);
   SA_CUDA(cudaGetLastError());
-  rc = do_search(e, e->q_bf16, nq, k, out_score_dev, out_idx_dev, out_score64_dev, nullptr, 0, st);
+  rc = do_search(e, e->q_bf16, nq, k, out_score_dev, out_idx_dev, out_score64_dev, nullptr, 0, st, filters);
   if (rc == SA_OK) e->ring[(e->n_searches - 1) % kTimingRing].kernels += 1;
   return rc;
+}
+
+int sa_search_f32(sa_engine* e, const float* q_f32_dev, int nq, int k, float* out_score_dev, int32_t* out_idx_dev,
+                  double* out_score64_dev, uintptr_t stream) {
+  return search_f32(e, q_f32_dev, nullptr, nq, k, out_score_dev, out_idx_dev, out_score64_dev, stream);
+}
+
+int sa_search_f32_filtered(sa_engine* e, const float* q_f32_dev, const sa_filter* filters_dev, int nq, int k,
+                           float* out_score_dev, int32_t* out_idx_dev, double* out_score64_dev, uintptr_t stream) {
+  int rc = check_engine(e);
+  if (rc) return rc;
+  rc = check_filtered(e, filters_dev);
+  if (rc) return rc;
+  return search_f32(e, q_f32_dev, reinterpret_cast<const sa::Filter*>(filters_dev), nq, k, out_score_dev, out_idx_dev,
+                    out_score64_dev, stream);
 }
 
 namespace {
@@ -1012,10 +1088,10 @@ int comm_gather_buffer(sa_comm* c, int local, int nq, int k, sa::PackedHit** out
 // must follow it on the stream may be issued before the group closes).
 int sharded_search_on_stream(sa_comm* c, int local, sa_engine* e, const uint16_t* q_bf16, int nq, int k,
                              int64_t row_offset, float* out_score_dev, long long* out_row_dev, cudaStream_t st,
-                             int phases = 7) {
+                             int phases = 7, const sa::Filter* filters = nullptr) {
   int rc;
   if (phases & 1) {
-    rc = do_search(e, q_bf16, nq, k, e->res_score, e->res_idx, nullptr, e->hits, row_offset, st);
+    rc = do_search(e, q_bf16, nq, k, e->res_score, e->res_idx, nullptr, e->hits, row_offset, st, filters);
     if (rc) return rc;
   }
   sa::PackedHit* gathered = nullptr;
@@ -1044,9 +1120,10 @@ int convert_queries(sa_engine* e, const float* q_f32_dev, int nq, cudaStream_t s
 
 // Host-buffer search into slot si.  comm == nullptr: this engine alone (shard-local int32 rows); otherwise this rank's
 // part of a sharded search (global int64 rows, identical on every rank).  `phases` as in sharded_search_on_stream
-// (bit 0 also covers the H2D copy and the conversion, bit 2 the D2H copies and the slot's event).
+// (bit 0 also covers the H2D copy and the conversion, bit 2 the D2H copies and the slot's event).  filters_host ([nq],
+// or nullptr: unfiltered) is staged through the slot's pinned buffer, so it may be reused as soon as submit returns.
 int host_submit(sa_engine* e, int si, const float* q_f32_host, int nq, int k, sa_comm* c, int local, int64_t row_offset,
-                int phases = 7) {
+                int phases = 7, const sa_filter* filters_host = nullptr) {
   sa_engine::HostSlot& sl = e->slot[si];
   SA_ON_DEVICE(e->device);
   cudaStream_t st = e->own_stream;
@@ -1065,15 +1142,22 @@ int host_submit(sa_engine* e, int si, const float* q_f32_host, int nq, int k, sa
       q_src = sl.h_q;
     }
     SA_CUDA(cudaMemcpyAsync(e->q_f32, q_src, qbytes, cudaMemcpyHostToDevice, st));
+    if (filters_host != nullptr) {
+      // the slot's device copy is read until the search's last kernel; the slot is not reused before its wait
+      memcpy(sl.h_f, filters_host, static_cast<size_t>(nq) * sizeof(sa::Filter));
+      SA_CUDA(cudaMemcpyAsync(sl.d_f, sl.h_f, static_cast<size_t>(nq) * sizeof(sa::Filter), cudaMemcpyHostToDevice, st));
+    }
     int rc = convert_queries(e, e->q_f32, nq, st);
     if (rc) return rc;
     if (c == nullptr) {
-      rc = do_search(e, e->q_bf16, nq, k, e->res_score, e->res_idx, nullptr, nullptr, 0, st);
+      rc = do_search(e, e->q_bf16, nq, k, e->res_score, e->res_idx, nullptr, nullptr, 0, st,
+                     filters_host != nullptr ? sl.d_f : nullptr);
       if (rc) return rc;
     }
   }
   if (c != nullptr) {
-    int rc = sharded_search_on_stream(c, local, e, e->q_bf16, nq, k, row_offset, e->res_score, e->res_row64, st, phases);
+    int rc = sharded_search_on_stream(c, local, e, e->q_bf16, nq, k, row_offset, e->res_score, e->res_row64, st, phases,
+                                      filters_host != nullptr ? sl.d_f : nullptr);
     if (rc) return rc;
   }
   if (phases & 4) {
@@ -1118,11 +1202,34 @@ int sa_search_host(sa_engine* e, const float* q_f32_host, int nq, int k, float* 
   return host_wait(e, kHostSlots, out_score_host, out_idx_host, false);
 }
 
+int sa_search_host_filtered(sa_engine* e, const float* q_f32_host, const sa_filter* filters_host, int nq, int k,
+                            float* out_score_host, int32_t* out_idx_host) {
+  int rc = check_engine(e);
+  if (rc) return rc;
+  rc = check_filtered(e, filters_host);
+  if (rc) return rc;
+  if (!out_score_host || !out_idx_host) return fail(SA_ERR_ARG, "null buffer");
+  e->slot[kHostSlots].busy = false;  // the private slot of the blocking call
+  rc = host_submit(e, kHostSlots, q_f32_host, nq, k, nullptr, 0, 0, 7, filters_host);
+  if (rc) return rc;
+  return host_wait(e, kHostSlots, out_score_host, out_idx_host, false);
+}
+
 int sa_search_host_submit(sa_engine* e, int slot, const float* q_f32_host, int nq, int k) {
   int rc = check_engine(e);
   if (rc) return rc;
   if (slot < 0 || slot >= kHostSlots) return fail(SA_ERR_ARG, "slot %d outside [0, %d)", slot, kHostSlots);
   return host_submit(e, slot, q_f32_host, nq, k, nullptr, 0, 0);
+}
+
+int sa_search_host_submit_filtered(sa_engine* e, int slot, const float* q_f32_host, const sa_filter* filters_host, int nq,
+                                   int k) {
+  int rc = check_engine(e);
+  if (rc) return rc;
+  rc = check_filtered(e, filters_host);
+  if (rc) return rc;
+  if (slot < 0 || slot >= kHostSlots) return fail(SA_ERR_ARG, "slot %d outside [0, %d)", slot, kHostSlots);
+  return host_submit(e, slot, q_f32_host, nq, k, nullptr, 0, 0, 7, filters_host);
 }
 
 int sa_search_host_wait(sa_engine* e, int slot, float* out_score_host, int32_t* out_idx_host) {
@@ -1157,6 +1264,23 @@ int sa_search_hits(sa_engine* e, const void* q_bf16_dev, int nq, int k, int64_t 
   }
   return do_search(e, static_cast<const uint16_t*>(q_bf16_dev), nq, k, e->res_score, e->res_idx, nullptr,
                    reinterpret_cast<sa::PackedHit*>(out_hits_dev), row_offset, st);
+}
+
+int sa_search_hits_filtered(sa_engine* e, const void* q_bf16_dev, const sa_filter* filters_dev, int nq, int k,
+                            int64_t row_offset, sa_hit* out_hits_dev, uintptr_t stream) {
+  int rc = check_engine(e);
+  if (rc) return rc;
+  rc = check_filtered(e, filters_dev);
+  if (rc) return rc;
+  if (!out_hits_dev) return fail(SA_ERR_ARG, "null buffer");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  {
+    SA_ON_DEVICE(e->device);
+    SA_CUDA(cudaStreamWaitEvent(st, e->scratch_free, 0));  // res_score / res_idx below are engine scratch
+  }
+  return do_search(e, static_cast<const uint16_t*>(q_bf16_dev), nq, k, e->res_score, e->res_idx, nullptr,
+                   reinterpret_cast<sa::PackedHit*>(out_hits_dev), row_offset, st,
+                   reinterpret_cast<const sa::Filter*>(filters_dev));
 }
 
 int sa_merge_hits(sa_engine* e, const sa_hit* hits_dev, int n_shards, int nq, int k, float* out_score_dev,
@@ -1299,6 +1423,23 @@ int sa_sharded_search(sa_comm* c, sa_engine* e, const void* q_bf16_dev, int nq, 
                                   reinterpret_cast<long long*>(out_row_dev), st);
 }
 
+int sa_sharded_search_filtered(sa_comm* c, sa_engine* e, const void* q_bf16_dev, const sa_filter* filters_dev, int nq,
+                               int k, int64_t row_offset, float* out_score_dev, int64_t* out_row_dev, uintptr_t stream) {
+  int rc = check_engine(e);
+  if (rc) return rc;
+  rc = check_filtered(e, filters_dev);
+  if (rc) return rc;
+  rc = check_rank_comm(c, e);
+  if (rc) return rc;
+  if (!out_score_dev || !out_row_dev) return fail(SA_ERR_ARG, "null buffer");
+  SA_ON_DEVICE(e->device);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  SA_CUDA(cudaStreamWaitEvent(st, e->scratch_free, 0));
+  return sharded_search_on_stream(c, 0, e, static_cast<const uint16_t*>(q_bf16_dev), nq, k, row_offset, out_score_dev,
+                                  reinterpret_cast<long long*>(out_row_dev), st, 7,
+                                  reinterpret_cast<const sa::Filter*>(filters_dev));
+}
+
 int sa_sharded_search_host_submit(sa_comm* c, sa_engine* e, int slot, const float* q_f32_host, int nq, int k,
                                   int64_t row_offset) {
   int rc = check_engine(e);
@@ -1309,6 +1450,18 @@ int sa_sharded_search_host_submit(sa_comm* c, sa_engine* e, int slot, const floa
   return host_submit(e, slot, q_f32_host, nq, k, c, 0, row_offset);
 }
 
+int sa_sharded_search_host_submit_filtered(sa_comm* c, sa_engine* e, int slot, const float* q_f32_host,
+                                           const sa_filter* filters_host, int nq, int k, int64_t row_offset) {
+  int rc = check_engine(e);
+  if (rc) return rc;
+  rc = check_filtered(e, filters_host);
+  if (rc) return rc;
+  rc = check_rank_comm(c, e);
+  if (rc) return rc;
+  if (slot < 0 || slot >= kHostSlots) return fail(SA_ERR_ARG, "slot %d outside [0, %d)", slot, kHostSlots);
+  return host_submit(e, slot, q_f32_host, nq, k, c, 0, row_offset, 7, filters_host);
+}
+
 int sa_sharded_search_host_wait(sa_comm* c, sa_engine* e, int slot, float* out_score_host, int64_t* out_row_host) {
   int rc = check_engine(e);
   if (rc) return rc;
@@ -1317,8 +1470,8 @@ int sa_sharded_search_host_wait(sa_comm* c, sa_engine* e, int slot, float* out_s
   return host_wait(e, slot, out_score_host, out_row_host, true);
 }
 
-int sa_gather_merge_submit(sa_comm* c, sa_engine* const* engines, int slot, const float* q_f32_host, int nq, int k,
-                           const int64_t* shard_offsets) {
+static int gather_merge_submit(sa_comm* c, sa_engine* const* engines, int slot, const float* q_f32_host,
+                               const sa_filter* filters_host, int nq, int k, const int64_t* shard_offsets) {
   if (!c || !engines || !shard_offsets) return fail(SA_ERR_ARG, "null argument");
   if (c->rank >= 0) return fail(SA_ERR_ARG, "multi-process communicator: use sa_sharded_search*");
   if (slot < 0 || slot >= kHostSlots) return fail(SA_ERR_ARG, "slot %d outside [0, %d)", slot, kHostSlots);
@@ -1329,12 +1482,16 @@ int sa_gather_merge_submit(sa_comm* c, sa_engine* const* engines, int slot, cons
       return fail(SA_ERR_ARG, "engine %d is on device %d, communicator rank %d on %d", g, engines[g]->device, g, c->devices[g]);
     if (engines[g]->sim != engines[0]->sim)
       return fail(SA_ERR_ARG, "engine %d has similarity %d, engine 0 has %d", g, engines[g]->sim, engines[0]->sim);
+    if (filters_host != nullptr) {
+      rc = check_filtered(engines[g], filters_host);
+      if (rc) return rc;
+    }
   }
   // every GPU gets the query block and runs the identical single-GPU path; the collectives of all local ranks are
   // issued inside one NCCL group (a single thread drives all devices)
   int rc = SA_OK;
   for (int g = 0; g < c->n_ranks; ++g) {
-    rc = host_submit(engines[g], slot, q_f32_host, nq, k, c, g, shard_offsets[g], 1);
+    rc = host_submit(engines[g], slot, q_f32_host, nq, k, c, g, shard_offsets[g], 1, filters_host);
     if (rc) return rc;
   }
   SA_NCCL(g_nccl.GroupStart());
@@ -1348,6 +1505,17 @@ int sa_gather_merge_submit(sa_comm* c, sa_engine* const* engines, int slot, cons
     if (rc) return rc;
   }
   return SA_OK;
+}
+
+int sa_gather_merge_submit(sa_comm* c, sa_engine* const* engines, int slot, const float* q_f32_host, int nq, int k,
+                           const int64_t* shard_offsets) {
+  return gather_merge_submit(c, engines, slot, q_f32_host, nullptr, nq, k, shard_offsets);
+}
+
+int sa_gather_merge_submit_filtered(sa_comm* c, sa_engine* const* engines, int slot, const float* q_f32_host,
+                                    const sa_filter* filters_host, int nq, int k, const int64_t* shard_offsets) {
+  if (!filters_host) return fail(SA_ERR_ARG, "null filters");
+  return gather_merge_submit(c, engines, slot, q_f32_host, filters_host, nq, k, shard_offsets);
 }
 
 int sa_gather_merge_wait(sa_comm* c, sa_engine* const* engines, int slot, float* out_score_host, int64_t* out_row_host) {
@@ -1369,6 +1537,13 @@ int sa_gather_merge_wait(sa_comm* c, sa_engine* const* engines, int slot, float*
 int sa_gather_merge(sa_comm* c, sa_engine* const* engines, const float* q_f32_host, int nq, int k,
                     const int64_t* shard_offsets, float* out_score_host, int64_t* out_row_host) {
   int rc = sa_gather_merge_submit(c, engines, 0, q_f32_host, nq, k, shard_offsets);
+  if (rc) return rc;
+  return sa_gather_merge_wait(c, engines, 0, out_score_host, out_row_host);
+}
+
+int sa_gather_merge_filtered(sa_comm* c, sa_engine* const* engines, const float* q_f32_host, const sa_filter* filters_host,
+                             int nq, int k, const int64_t* shard_offsets, float* out_score_host, int64_t* out_row_host) {
+  int rc = sa_gather_merge_submit_filtered(c, engines, 0, q_f32_host, filters_host, nq, k, shard_offsets);
   if (rc) return rc;
   return sa_gather_merge_wait(c, engines, 0, out_score_host, out_row_host);
 }
@@ -1519,6 +1694,7 @@ int sa_get_info(const sa_engine* e, const char* name, int64_t* value) {
   else if (!strcmp(name, "last_fix_entries")) *value = e->last_fix_entries;
   else if (!strcmp(name, "eps_rel_e12")) *value = static_cast<int64_t>(static_cast<double>(scan_eps_rel(e->dim)) * 1e12);
   else if (!strcmp(name, "similarity")) *value = e->sim;
+  else if (!strcmp(name, "has_tags")) *value = e->row_tags != nullptr ? 1 : 0;
   else if (!strcmp(name, "cmax_bits")) {
     unsigned bits = 0;
     DeviceGuard dg(e->device);
@@ -1647,6 +1823,13 @@ int sa_debug_window_bound(const uint32_t* keys, int n_windows, int list_len, uin
     if (out_sorted)
       for (int i = 0; i < sa::kWin; ++i) out_sorted[static_cast<size_t>(w) * sa::kWin + i] = x[i];
   }
+  return SA_OK;
+}
+
+int sa_debug_filter_pass(const uint64_t* tags, int n, const sa_filter* f, uint8_t* out) {
+  if (!tags || !f || !out || n < 0) return fail(SA_ERR_ARG, "bad argument");
+  const sa::Filter& F = *reinterpret_cast<const sa::Filter*>(f);
+  for (int i = 0; i < n; ++i) out[i] = sa::filter_pass(tags[i], F) ? 1 : 0;
   return SA_OK;
 }
 

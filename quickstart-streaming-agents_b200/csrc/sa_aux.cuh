@@ -189,6 +189,18 @@ __global__ void sa_convert_rows_term_kernel(const float* __restrict__ src, uint1
   block_raise_cmax(cmax, &blk_max, nb, active && lane == 0);
 }
 
+// Per-query filter over the rows' 64-bit tags (sa_filter of sa_api.h, same layout).  One definition of the predicate
+// serves the scan's epilogue, the exact fallback scan and the host test hook (sa_debug_filter_pass).
+struct Filter {
+  unsigned long long all_of;     // every bit must be set on the row
+  unsigned long long none_of;    // no bit may be set
+  unsigned long long any_of[2];  // each nonzero word: at least one of its bits must be set
+};
+__host__ __device__ __forceinline__ bool filter_pass(unsigned long long t, const Filter& f) {
+  return ((t & f.all_of) == f.all_of) & ((t & f.none_of) == 0ull) & ((f.any_of[0] == 0ull) | ((t & f.any_of[0]) != 0ull)) &
+         ((f.any_of[1] == 0ull) | ((t & f.any_of[1]) != 0ull));
+}
+
 // Order-preserving map: (score desc, row asc)  <=>  key desc.
 __host__ __device__ __forceinline__ unsigned long long make_key(float s, int row) {
   uint32_t u = aux_f32_bits(s);
@@ -521,6 +533,8 @@ struct FixParams {
   int zero_b_n;
   unsigned* zero_c;         // ... and the lanes' second-best table (window bound)
   int zero_c_n;
+  const unsigned long long* row_tags;  // filtered search: [capacity] the rows' tags ...
+  const Filter* filters;               // ... and [nq] the queries' filters; nullptr: unfiltered
 };
 
 constexpr int kFixThreads = 256;
@@ -596,6 +610,8 @@ __global__ void __launch_bounds__(kFixThreads) sa_fixup_kernel(const FixParams p
     volatile double* g_cos = p.res64 + static_cast<size_t>(en.q) * p.k;
     volatile int* g_row = p.residx + static_cast<size_t>(en.q) * p.k;
     const uint4* qv = reinterpret_cast<const uint4*>(p.queries + static_cast<size_t>(en.q) * p.dim);
+    Filter flt = {0ull, 0ull, {0ull, 0ull}};  // match-all unless the search is filtered
+    if (p.filters != nullptr) flt = p.filters[en.q];
 
     __syncthreads();  // previous item's smem no longer in use
     for (int i = tid; i < nvec; i += kFixThreads) {
@@ -629,6 +645,7 @@ __global__ void __launch_bounds__(kFixThreads) sa_fixup_kernel(const FixParams p
         if (r >= p.n_rows) break;
         const float wr = __ldg(p.row_term + r);
         if (p.sim == kSimEuc ? !(wr >= 0.f) : !(wr > 0.f)) continue;  // rows that are not live are never returned
+        if (p.filters != nullptr && !filter_pass(__ldg(p.row_tags + r), flt)) continue;  // nor rows the filter excludes
         const uint4* cv = reinterpret_cast<const uint4*>(p.corpus + static_cast<size_t>(r) * p.dim);
         float acc = 0.f;
         for (int i = lane; i < nvec; i += 32) {

@@ -11,6 +11,8 @@
 //   dotProduct  v = acc * w, w = 1         (0 = tombstone)         kEpi = kEpiMul  (the cosine instantiations, unchanged)
 //   euclidean   v = acc - w, w = |c|^2 / 2 (negative = tombstone)  kEpi = kEpiSub
 // so v is always "larger is better": for euclidean v = <q,c> - |c|^2/2 = (|q|^2 - |q - c|^2) / 2.
+// A filtered search (kEpi | kEpiFilt) also masks, per query, the rows whose 64-bit tag fails the query's Filter: their row
+// term becomes NaN, exactly like a tombstone's, so an ineligible row never enters a list, raises `drop` or a threshold.
 //
 // Nothing but the per-CTA candidate lists (kKL entries per query, plus one "dropped" bound per query) leaves the SM.
 //
@@ -27,6 +29,7 @@
 // bound shared between lanes).  The merge kernel turns (lists, drops) into either a certificate that the exactly
 // re-scored candidates contain the true top-k, or a work item for the exact fallback scan.
 #pragma once
+#include "sa_aux.cuh"
 #include "sm90_ptx.cuh"
 #include <cmath>
 #include <cstring>
@@ -55,8 +58,9 @@ constexpr int kModeProf = 2;   // profiling: per-role wait / busy cycle counters
 // kEpi of the scan kernel: how the accumulator and the row term combine (see the header comment)
 constexpr int kEpiMul = 0;     // v = acc * w; a row is live iff w > 0 (cosine, dotProduct)
 constexpr int kEpiSub = 1;     // v = acc - w; a row is live iff w >= 0 (euclidean)
+constexpr int kEpiFilt = 2;    // flag: filtered search (ScanParams::row_tags / filters)
 
-template <int kCG>
+template <int kCG, bool kFilt = false>
 struct ScanCfg {
   static constexpr int kStages = 3;
   static constexpr int kBRows = kBlockN / kCG;  // corpus rows of a tile loaded (and multicast) by each CTA
@@ -67,9 +71,12 @@ struct ScanCfg {
   static constexpr uint32_t kStagingBytes = kBlockM * kStagingLd * sizeof(float);
   static constexpr uint32_t kIcBytes = 4 * kBlockN * sizeof(float);  // one 256-float scale vector per epilogue warp
   static constexpr uint32_t kBarBytes = 2 * kStages * 8;
+  // filtered search: one 256-tag vector per epilogue warp, after the barriers (the unfiltered layout is unchanged)
+  static constexpr uint32_t kTagBytes = kFilt ? 4 * kBlockN * sizeof(unsigned long long) : 0;
   // +1024: the dynamic smem base is aligned up to 1024 B by hand (SWIZZLE_128B requirement).
-  static constexpr uint32_t kSmemBytes = kStages * kStageBytes + kStagingBytes + kIcBytes + kBarBytes + 1024;
+  static constexpr uint32_t kSmemBytes = kStages * kStageBytes + kStagingBytes + kIcBytes + kBarBytes + kTagBytes + 1024;
   static_assert(kSmemBytes <= 227 * 1024, "H100 allows 227 KB of shared memory per block");
+  static_assert(!kFilt || kSmemBytes == 228400, "filtered scan: the unfiltered 220 208 B plus 8 KB of tags");
 };
 
 // Per-CTA profile record (kModeProf): SM cycles, summed over the kernel.
@@ -113,6 +120,8 @@ struct ScanParams {
   float* dbg_dots;        // kModeDots only: raw accumulators of (unit 0 .. nqb-1, tile dbg_tile) [nqb*128*kCG][256]
   int dbg_tile;
   ScanProf* prof;         // kModeProf only: [gridDim.x]
+  const unsigned long long* row_tags;  // kEpiFilt only: [capacity] the rows' tags, 16-byte aligned (rows < n_rows read)
+  const Filter* filters;               // kEpiFilt only: [nq] this launch's queries' filters
 };
 
 // Bit casts usable on both sides of the compiler: the device path is the intrinsic, the host path (used only by the
@@ -320,13 +329,23 @@ __host__ __device__ __forceinline__ bool chunk_process(TopList<kKL>& L, float (&
 #ifdef __CUDACC__
 // Epilogue of one half tile: 128 columns of this thread's query row in the staging buffer -> scaled scores -> list.
 // `ic` is this warp's private 256-float scale vector of the tile in shared memory (broadcast reads).
+// Filtered (kEpi & kEpiFilt): `tg` is the warp's tag vector of the half, and a row failing the thread's filter `*fp`
+// gets the row term NaN (acc * NaN and acc - NaN are NaN: masked like a tombstone).  The filter is re-read (L1) and
+// reduced to a 32-bit pass mask per chunk before the chunk's values are loaded, so it holds no registers in between.
 template <int kKL, int kMode, int kEpi>
 __device__ __forceinline__ int epilogue_half(TopList<kKL>& L, const float* srow, const float* ic, int row0,
-                                             float* dbg_row) {
+                                             float* dbg_row, const unsigned long long* tg = nullptr,
+                                             const Filter* fp = nullptr) {
   int slow = 0;
   float v[kChunk], w[kChunk];
 #pragma unroll 1
   for (int c = 0; c < kHalfN / kChunk; ++c) {
+    unsigned pass = 0u;
+    if constexpr ((kEpi & kEpiFilt) != 0) {
+      const Filter F = *fp;
+#pragma unroll
+      for (int j = 0; j < kChunk; ++j) pass |= filter_pass(tg[c * kChunk + j], F) ? (1u << j) : 0u;
+    }
     const float4* s4 = reinterpret_cast<const float4*>(srow + c * kChunk);
     const float4* w4 = reinterpret_cast<const float4*>(ic + c * kChunk);
 #pragma unroll
@@ -341,13 +360,18 @@ __device__ __forceinline__ int epilogue_half(TopList<kKL>& L, const float* srow,
       w[4 * i + 2] = y.z;
       w[4 * i + 3] = y.w;
     }
+    if constexpr ((kEpi & kEpiFilt) != 0) {
+      const float qnan = __int_as_float(0x7fc00000);
+#pragma unroll
+      for (int j = 0; j < kChunk; ++j) w[j] = ((pass >> j) & 1u) ? w[j] : qnan;
+    }
     if constexpr (kMode == kModeDots) {
       if (dbg_row != nullptr) {
 #pragma unroll
         for (int j = 0; j < kChunk; ++j) dbg_row[c * kChunk + j] = v[j];
       }
     }
-    slow += chunk_process<kKL, kEpi>(L, v, w, row0 + c * kChunk) ? 1 : 0;
+    slow += chunk_process<kKL, kEpi & 1>(L, v, w, row0 + c * kChunk) ? 1 : 0;
     __syncwarp();  // reconverge after the divergent insertion path
   }
   return slow;
@@ -357,7 +381,8 @@ template <int kCG, int kKL, int kMode, int kEpi = kEpiMul>
 __global__ void __launch_bounds__(kScanThreads, 1)
 sa_scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_c,
                const ScanParams p) {
-  using Cfg = ScanCfg<kCG>;
+  constexpr bool kFilt = (kEpi & kEpiFilt) != 0;
+  using Cfg = ScanCfg<kCG, kFilt>;
   constexpr int kStages = Cfg::kStages;
   constexpr int kRowsPerQb = kBlockM * kCG;
   constexpr bool kProf = (kMode == kModeProf);
@@ -373,6 +398,7 @@ sa_scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant
   auto empty_bar = [&](int s) { return bar_base + 8u * (kStages + s); };
   auto a_smem = [&](int s) { return smem_base + s * Cfg::kStageBytes; };
   auto b_smem = [&](int s) { return smem_base + s * Cfg::kStageBytes + Cfg::kABytes; };
+  const uint32_t tag_base = bar_base + Cfg::kBarBytes;  // [4][256] tags (kFilt only)
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -508,7 +534,7 @@ sa_scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant
     // and rows that are not live (all-zero rows under cosine, tombstones) with NaN (NaN never compares greater than a
     // threshold, so they cannot enter a list and are ignored by every max), and the warp shares them through its
     // private smem vector.  Past the prefix the term reads as kPast, which every epilogue masks.
-    constexpr float kPast = (kEpi == kEpiSub) ? -1.f : 0.f;
+    constexpr float kPast = ((kEpi & 1) == kEpiSub) ? -1.f : 0.f;
     float4 nx0 = make_float4(0.f, 0.f, 0.f, 0.f), nx1 = nx0;
     auto fetch_ic = [&](int t) {
       const long long r0 = static_cast<long long>(t) * kBlockN + 8 * lane;
@@ -525,6 +551,22 @@ sa_scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant
       }
     };
     if (epi && tl < walk_tiles) fetch_ic(tl * p.tile_stride);
+    // Tags of tile t (kFilt): lane l copies rows [8l, 8l+8) into the warp's private vector with cp.async, issued once
+    // the warp's previous epilogue is done with the vector and waited for at the start of the next epilogue, so the
+    // copy holds no registers across the MMAs.  Tags at or past n_rows are not read (zero-filled; those rows are masked).
+    auto fetch_tags = [&](int t) {
+      const long long r0 = static_cast<long long>(t) * kBlockN + 8 * lane;
+      const uint32_t dst = tag_base + static_cast<uint32_t>((ew * kBlockN + 8 * lane) * sizeof(unsigned long long));
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const long long left = p.n_rows - (r0 + 2 * j);
+        const uint32_t bytes = left >= 2 ? 16u : (left == 1 ? 8u : 0u);
+        cp_async_16(dst + 16u * j, p.row_tags + (bytes != 0u ? r0 + 2 * j : 0), bytes);
+      }
+    };
+    if constexpr (kFilt) {
+      if (epi && tl < walk_tiles) fetch_tags(tl * p.tile_stride);
+    }
 
     // Window bound (see window_bound): this thread's slot in the lanes' second-best table, and the kWin lanes it reads.
     const bool win_on = p.lane2 != nullptr && TL >= kWin && own_query;
@@ -553,7 +595,7 @@ sa_scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant
         L.apply_shared(L.nxt_key);
         const float qnan = __int_as_float(0x7fc00000);
         auto sc = [&](float x) {
-          if constexpr (kEpi == kEpiSub)
+          if constexpr ((kEpi & 1) == kEpiSub)
             return x >= 0.f ? x : qnan;
           else
             return x > 0.f ? x : qnan;
@@ -638,9 +680,24 @@ sa_scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant
         named_bar_sync(named_bar, 128);
         long long c2 = 0;
         if constexpr (kProf) c2 = clock64();
-        if (epi)
+        if constexpr (kFilt) {
+          if (epi && h == 0) {
+            cp_async_wait_all();
+            __syncwarp();  // every lane's tags of this tile are in the warp's vector
+          }
+        }
+        if constexpr (kFilt) {
+          // this warp's tag vector, formed here rather than held across the MMAs
+          const unsigned long long* tg =
+              reinterpret_cast<const unsigned long long*>(smem_gen + (tag_base - smem_base)) + ew * kBlockN;
+          if (epi)
+            slow += epilogue_half<kKL, kMode, kEpi>(L, stg + wt * kStagingLd, ic + h * kHalfN, t * kBlockN + h * kHalfN,
+                                                    dbg_row != nullptr ? dbg_row + h * kHalfN : nullptr, tg + h * kHalfN,
+                                                    p.filters + (own_query ? query : 0));
+        } else if (epi) {
           slow += epilogue_half<kKL, kMode, kEpi>(L, stg + wt * kStagingLd, ic + h * kHalfN, t * kBlockN + h * kHalfN,
                                                   dbg_row != nullptr ? dbg_row + h * kHalfN : nullptr);
+        }
         if constexpr (kProf) {
           w_stage += c2 - c1;
           busy += clock64() - c2;
@@ -648,6 +705,12 @@ sa_scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant
       };
       stage_and_score(acc0, 0);
       stage_and_score(acc1, 1);
+      if constexpr (kFilt) {
+        if (epi && ti + TL < walk_tiles) {
+          __syncwarp();  // every lane is done reading this tile's tags
+          fetch_tags((ti + TL) * p.tile_stride);
+        }
+      }
       if constexpr (kProf) slow_chunks += slow;
       if (epi) {
         if (L.slot != nullptr) {

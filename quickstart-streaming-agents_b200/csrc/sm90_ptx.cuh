@@ -123,6 +123,15 @@ __device__ __forceinline__ void st_relaxed_gpu_u32(unsigned* p, unsigned v) {
 }
 
 // ----------------------------------------------------------------------------------------------
+// cp.async: 16-byte global -> shared copies that hold no registers until they are waited for
+// ----------------------------------------------------------------------------------------------
+// src_bytes < 16 reads only that many bytes and zero-fills the rest (0: nothing is read)
+__device__ __forceinline__ void cp_async_16(uint32_t dst, const void* src, uint32_t src_bytes) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
+}
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
+
+// ----------------------------------------------------------------------------------------------
 // Cluster
 // ----------------------------------------------------------------------------------------------
 __device__ __forceinline__ void cluster_sync_all() {

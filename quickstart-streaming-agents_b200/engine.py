@@ -33,6 +33,20 @@ def _ptr(t: torch.Tensor | None) -> int:
 HIT_DTYPE = np.dtype([("score", "<f8"), ("row", "<i8")])   # sa_hit of include/sa_api.h
 
 
+def filter_array(filters, nq: int) -> np.ndarray:
+    """Per-query filters (sa_filter of include/sa_api.h: all_of, none_of, any_of[0], any_of[1]) as a contiguous uint64
+    array [nq, 4]; one filter of shape [4] applies to every query."""
+    f = np.asarray(filters)
+    if f.dtype.kind not in "iu":
+        raise TypeError("filters must be an integer array of uint64 words")
+    f = f.astype(np.uint64) if f.dtype != np.uint64 else f
+    if f.shape == (4,):
+        f = np.broadcast_to(f, (nq, 4))
+    if f.shape != (nq, 4):
+        raise ValueError(f"filters must have shape [4] or [nq={nq}, 4], not {list(f.shape)}")
+    return np.ascontiguousarray(f)
+
+
 def pinned_array(shape, dtype=np.float32) -> np.ndarray:
     """A page-locked numpy array (sa_host_alloc), freed (sa_host_free) when its last view is garbage-collected."""
     import weakref
@@ -51,7 +65,10 @@ class VectorIndex:
     ``similarity`` is the Atlas index setting, fixed at creation: "cosine" (default), "dotProduct" or "euclidean"
     (include/sa_api.h, SA_SIM_*).  Scores are cosines, dot products or Euclidean distances accordingly; results are
     ordered best first (ascending distance for "euclidean").  ``inv_norm`` holds the row terms: 1/|c| for cosine, 1 for
-    dotProduct, |c|^2/2 for euclidean."""
+    dotProduct, |c|^2/2 for euclidean.
+
+    ``tags`` holds one 64-bit filter tag per row (uint64 bits in an int64 tensor [capacity]); the searches' ``filters``
+    argument restricts each query to the rows whose tag passes its filter (``filter_array``, qsa_b200.filters)."""
 
     def __init__(self, dim: int = 1536, capacity: int = 1 << 20, max_batch: int = 1024, max_k: int = 10,
                  device: int | None = None, similarity: str = "cosine"):
@@ -66,6 +83,7 @@ class VectorIndex:
         # device-memory holders (the engine never copies or frees these)
         self.rows = torch.empty((self.capacity, self.dim), dtype=torch.bfloat16, device=dev)
         self.inv_norm = torch.zeros((self.capacity,), dtype=torch.float32, device=dev)
+        self.tags = torch.zeros((self.capacity,), dtype=torch.int64, device=dev)
         h = C.c_void_p()
         capi.check(self.lib.sa_engine_create_sim(C.byref(h), self.device, self.dim, self.capacity, self.max_batch,
                                                  self.max_k, sim), "sa_engine_create_sim")
@@ -73,6 +91,7 @@ class VectorIndex:
         self._inflight = {}
         capi.check(self.lib.sa_corpus_bind(self._h, self.rows.data_ptr(), self.inv_norm.data_ptr(), 0),
                    "sa_corpus_bind")
+        capi.check(self.lib.sa_corpus_bind_tags(self._h, self.tags.data_ptr()), "sa_corpus_bind_tags")
 
     # ------------------------------------------------------------------ lifecycle
     def close(self) -> None:
@@ -107,26 +126,51 @@ class VectorIndex:
         """Forget every row (the job of scripts/common/clear_mongodb.py:98-158 in the reference)."""
         capi.check(self.lib.sa_corpus_reset(self._h), "sa_corpus_reset")
 
-    def append(self, rows_f32) -> int:
-        """Append fp32 embeddings (host numpy or device tensor) -> bf16 rows + norms.  Returns first row id."""
+    def _write_tags(self, first: int, n: int, tags) -> None:
+        """Tags of rows [first, first + n): the given uint64 words, or zeros.  Written before the rows are committed."""
+        if first + n > self.capacity:
+            raise capi.SaError(capi.SA_ERR_CAPACITY, "tags", "append past capacity")
+        if tags is None:
+            self.tags[first:first + n].zero_()
+            return
+        t = np.ascontiguousarray(tags, dtype=np.uint64)
+        if t.shape != (n,):
+            raise ValueError(f"tags must have shape [{n}], not {list(t.shape)}")
+        self.tags[first:first + n].copy_(torch.from_numpy(t.view(np.int64)))
+
+    def set_tags(self, rows, tags) -> None:
+        """Rewrite the tags of committed rows (between searches)."""
+        ix = torch.as_tensor(np.asarray(rows, dtype=np.int64), device=self.tags.device)
+        t = np.ascontiguousarray(tags, dtype=np.uint64)
+        if t.shape != (len(ix),):
+            raise ValueError(f"tags must have shape [{len(ix)}], not {list(t.shape)}")
+        if len(ix) and (int(ix.min()) < 0 or int(ix.max()) >= len(self)):
+            raise IndexError("set_tags: row outside the committed rows")
+        self.tags[ix] = torch.from_numpy(t.view(np.int64)).to(self.tags.device)
+
+    def append(self, rows_f32, tags=None) -> int:
+        """Append fp32 embeddings (host numpy or device tensor) -> bf16 rows + norms.  Returns first row id.
+        ``tags`` (uint64 [n]) are the new rows' filter tags; without them the rows get tag 0."""
         first = len(self)
         if isinstance(rows_f32, torch.Tensor) and rows_f32.is_cuda:
             x = rows_f32.to(torch.float32).contiguous()
             assert x.dim() == 2 and x.shape[1] == self.dim
+            self._write_tags(first, x.shape[0], tags)
             capi.check(self.lib.sa_corpus_append_f32(self._h, x.data_ptr(), x.shape[0], self._stream()),
                        "sa_corpus_append_f32")
             torch.cuda.current_stream(self.device).synchronize()  # x may be freed by the caller
         else:
             x = np.ascontiguousarray(rows_f32, dtype=np.float32)
             assert x.ndim == 2 and x.shape[1] == self.dim
+            self._write_tags(first, x.shape[0], tags)
             torch.cuda.current_stream(self.device).synchronize()  # the *_host calls run on the engine's stream
             capi.check(self.lib.sa_corpus_append_host_f32(self._h, x.ctypes.data, x.shape[0]),
                        "sa_corpus_append_host_f32")
         return first
 
-    def append_bf16_bits(self, bits: np.ndarray) -> int:
+    def append_bf16_bits(self, bits: np.ndarray, tags=None) -> int:
         """Append rows given as bf16 bit patterns (uint16 [n, dim]) -- used with the synthetic corpora so the
-        device holds exactly the bits the oracle sees."""
+        device holds exactly the bits the oracle sees.  ``tags`` as in ``append``."""
         bits = np.ascontiguousarray(bits, dtype=np.uint16)
         assert bits.ndim == 2 and bits.shape[1] == self.dim
         first = len(self)
@@ -134,14 +178,15 @@ class VectorIndex:
         if first + n > self.capacity:
             raise capi.SaError(capi.SA_ERR_CAPACITY, "append_bf16_bits", "append past capacity")
         src = torch.from_numpy(bits.view(np.int16)).view(torch.bfloat16)
+        self._write_tags(first, n, tags)
         self.rows[first:first + n].copy_(src)
         self.commit(first, n)
         return first
 
     # ------------------------------------------------------------------ checkpoint / resume
     def snapshot(self, path: str) -> int:
-        """Write the committed rows (bf16 bits), their row terms and the similarity to ``path`` (.npz).  Returns the
-        row count.
+        """Write the committed rows (bf16 bits), their row terms, their filter tags and the similarity to ``path``
+        (.npz).  Returns the row count.
         (The reference leaves corpus durability to Atlas; here a snapshot + the consumer-group offsets are the
         checkpoint, and replaying `documents_embed` from offset 0 is the fallback.)"""
         n = len(self)
@@ -152,7 +197,7 @@ class VectorIndex:
         tmp = path + ".tmp"
         with open(tmp, "wb") as f:                       # written under a temporary name, then renamed: never half a file
             np.savez(f, rows=bits, inv_norm=self.inv_norm[:n].cpu().numpy(), dim=np.int64(self.dim),
-                     similarity=np.str_(self.similarity))
+                     similarity=np.str_(self.similarity), tags=self.tags[:n].cpu().numpy().view(np.uint64))
             f.flush()
             os.fsync(f.fileno())
         os.replace(tmp, path)
@@ -161,7 +206,7 @@ class VectorIndex:
     def restore(self, path: str) -> int:
         """Load a snapshot written by ``snapshot`` into this (empty or not) index, replacing its contents.  A snapshot
         without a recorded similarity is a cosine one; a snapshot of another similarity is refused (its row terms and
-        its rankings mean something else)."""
+        its rankings mean something else).  A snapshot without tags restores tag 0 on every row."""
         z = np.load(path if path.endswith(".npz") else path + ".npz")
         if int(z["dim"]) != self.dim:
             raise ValueError(f"snapshot has dim {int(z['dim'])}, index has {self.dim}")
@@ -174,6 +219,10 @@ class VectorIndex:
             raise capi.SaError(capi.SA_ERR_CAPACITY, "restore", "snapshot larger than capacity")
         self.rows[:n].copy_(torch.from_numpy(bits.view(np.int16)).view(torch.bfloat16))
         self.inv_norm[:n].copy_(torch.from_numpy(inv))
+        if "tags" in z.files:
+            self.tags[:n].copy_(torch.from_numpy(np.ascontiguousarray(z["tags"], dtype=np.uint64).view(np.int64)))
+        else:
+            self.tags[:n].zero_()
         torch.cuda.current_stream(self.device).synchronize()
         capi.check(self.lib.sa_corpus_bind(self._h, self.rows.data_ptr(), self.inv_norm.data_ptr(), n),
                    "sa_corpus_bind")
@@ -193,9 +242,13 @@ class VectorIndex:
         capi.check(self.lib.sa_corpus_commit(self._h, int(first), int(n), self._stream()), "sa_corpus_commit")
 
     # ------------------------------------------------------------------ search
-    def search(self, q: torch.Tensor, k: int, want_score64: bool = False):
+    def _filters_dev(self, filters, nq: int, dev) -> torch.Tensor:
+        return torch.from_numpy(filter_array(filters, nq).view(np.int64).copy()).to(dev)
+
+    def search(self, q: torch.Tensor, k: int, want_score64: bool = False, filters=None):
         """Device path.  q: [nq, dim] bf16 or fp32 CUDA tensor.  Returns (score f32 [nq,k], idx i32 [nq,k]
-        [, score64 f64 [nq,k]]) as CUDA tensors, asynchronous on the current stream."""
+        [, score64 f64 [nq,k]]) as CUDA tensors, asynchronous on the current stream.  ``filters`` (uint64 [nq, 4] or
+        [4], see ``filter_array``) restricts each query to the rows whose tag passes its filter."""
         assert q.is_cuda and q.dim() == 2 and q.shape[1] == self.dim
         q = q.contiguous()
         nq = q.shape[0]
@@ -203,6 +256,18 @@ class VectorIndex:
         score = torch.empty((nq, k), dtype=torch.float32, device=dev)
         idx = torch.empty((nq, k), dtype=torch.int32, device=dev)
         s64 = torch.empty((nq, k), dtype=torch.float64, device=dev) if want_score64 else None
+        if filters is not None:
+            f = self._filters_dev(filters, nq, dev)
+            if q.dtype == torch.bfloat16:
+                rc = self.lib.sa_search_filtered(self._h, q.data_ptr(), f.data_ptr(), nq, k, score.data_ptr(),
+                                                 idx.data_ptr(), _ptr(s64), self._stream())
+            elif q.dtype == torch.float32:
+                rc = self.lib.sa_search_f32_filtered(self._h, q.data_ptr(), f.data_ptr(), nq, k, score.data_ptr(),
+                                                     idx.data_ptr(), _ptr(s64), self._stream())
+            else:
+                raise TypeError("queries must be bf16 or fp32")
+            capi.check(rc, "sa_search_filtered")
+            return (score, idx, s64) if want_score64 else (score, idx)
         if q.dtype == torch.bfloat16:
             rc = self.lib.sa_search(self._h, q.data_ptr(), nq, k, score.data_ptr(), idx.data_ptr(), _ptr(s64),
                                     self._stream())
@@ -214,9 +279,10 @@ class VectorIndex:
         capi.check(rc, "sa_search")
         return (score, idx, s64) if want_score64 else (score, idx)
 
-    def search_host(self, q_f32: np.ndarray, k: int, out=None):
+    def search_host(self, q_f32: np.ndarray, k: int, out=None, filters=None):
         """End-to-end path with HOST buffers (H2D, search, D2H inside the call).  Returns numpy
-        (score f32 [nq,k], idx i32 [nq,k]); ``out=(score, idx)`` reuses caller buffers (e.g. ``pinned_array``)."""
+        (score f32 [nq,k], idx i32 [nq,k]); ``out=(score, idx)`` reuses caller buffers (e.g. ``pinned_array``).
+        ``filters`` as in ``search``."""
         q = np.ascontiguousarray(q_f32, dtype=np.float32)
         assert q.ndim == 2 and q.shape[1] == self.dim
         nq = q.shape[0]
@@ -228,17 +294,28 @@ class VectorIndex:
             assert score.shape == (nq, k) and score.dtype == np.float32 and score.flags.c_contiguous
             assert idx.shape == (nq, k) and idx.dtype == np.int32 and idx.flags.c_contiguous
         torch.cuda.current_stream(self.device).synchronize()  # the *_host calls run on the engine's stream
+        if filters is not None:
+            f = filter_array(filters, nq)
+            capi.check(self.lib.sa_search_host_filtered(self._h, q.ctypes.data, f.ctypes.data, nq, k, score.ctypes.data,
+                                                        idx.ctypes.data), "sa_search_host_filtered")
+            return score, idx
         capi.check(self.lib.sa_search_host(self._h, q.ctypes.data, nq, k, score.ctypes.data, idx.ctypes.data),
                    "sa_search_host")
         return score, idx
 
-    def search_host_submit(self, q_f32: np.ndarray, k: int, slot: int = 0) -> None:
+    def search_host_submit(self, q_f32: np.ndarray, k: int, slot: int = 0, filters=None) -> None:
         """First half of ``search_host``: enqueue H2D + search + D2H for ``slot`` (0 or 1) and return at once, so the
-        caller can prepare the next batch while the GPU works.  Collect with ``search_host_wait(slot)``."""
+        caller can prepare the next batch while the GPU works.  Collect with ``search_host_wait(slot)``.
+        ``filters`` as in ``search`` (staged by the call: the array may be reused at once)."""
         q = np.ascontiguousarray(q_f32, dtype=np.float32)
         assert q.ndim == 2 and q.shape[1] == self.dim
         torch.cuda.current_stream(self.device).synchronize()  # the *_host calls run on the engine's own stream
         self._inflight[slot] = (q, q.shape[0], k)  # keeps a pinned source alive until the wait
+        if filters is not None:
+            f = filter_array(filters, q.shape[0])
+            capi.check(self.lib.sa_search_host_submit_filtered(self._h, slot, q.ctypes.data, f.ctypes.data, q.shape[0],
+                                                               k), "sa_search_host_submit_filtered")
+            return
         capi.check(self.lib.sa_search_host_submit(self._h, slot, q.ctypes.data, q.shape[0], k),
                    "sa_search_host_submit")
 
@@ -260,12 +337,18 @@ class VectorIndex:
         them directly instead of staging through its own pinned copy.  Freed when the index is closed."""
         return pinned_array(shape, dtype)
 
-    def search_hits(self, q: torch.Tensor, k: int, row_offset: int = 0) -> torch.Tensor:
+    def search_hits(self, q: torch.Tensor, k: int, row_offset: int = 0, filters=None) -> torch.Tensor:
         """This shard's results in exchange format: uint8 CUDA tensor [nq, k, 16] = sa_hit {score f64, global row i64}
-        (``hits.view(torch.float64)[..., 0]`` / ``.view(torch.int64)[..., 1]``)."""
+        (``hits.view(torch.float64)[..., 0]`` / ``.view(torch.int64)[..., 1]``).  ``filters`` as in ``search``."""
         assert q.is_cuda and q.dtype == torch.bfloat16 and q.dim() == 2 and q.shape[1] == self.dim
         q = q.contiguous()
         hits = torch.empty((q.shape[0], k, 16), dtype=torch.uint8, device=q.device)
+        if filters is not None:
+            f = self._filters_dev(filters, q.shape[0], q.device)
+            capi.check(self.lib.sa_search_hits_filtered(self._h, q.data_ptr(), f.data_ptr(), q.shape[0], k,
+                                                        int(row_offset), hits.data_ptr(), self._stream()),
+                       "sa_search_hits_filtered")
+            return hits
         capi.check(self.lib.sa_search_hits(self._h, q.data_ptr(), q.shape[0], k, int(row_offset), hits.data_ptr(),
                                            self._stream()), "sa_search_hits")
         return hits

@@ -14,13 +14,17 @@ the embedding column lives in HBM inside a ``VectorIndex``, the other columns in
 ``search_results`` array of rows ``(table columns..., score)`` in descending score order.
 
 The index object only needs ``append(rows_f32) -> first_row``, ``search_host(q_f32, k) -> (score, idx)``,
-``reset()``, ``__len__`` and ``delete_rows`` -- production passes ``engine.VectorIndex`` (CUDA, no fallback).
+``reset()``, ``__len__`` and ``delete_rows`` -- production passes ``engine.VectorIndex`` (CUDA, no fallback).  A table
+with ``filter_fields`` (Atlas's ``{"type": "filter"}`` fields) also needs ``append(rows, tags=...)``, ``set_tags`` and
+``search_host(..., filters=...)``.
 """
 from __future__ import annotations
 
 from dataclasses import dataclass, field
 
 import numpy as np
+
+from .filters import FilterSchema, compile_filter
 
 
 def _avro_nullable_string(v: str | None) -> bytes:
@@ -97,10 +101,16 @@ class SearchHit:
 
 
 class VectorTable:
-    def __init__(self, index, name: str = "documents_vectordb_lab2", embedding_column: str = "embedding"):
+    """``filter_fields``: the metadata columns declared as Atlas filter fields; their values become the rows' tags, and
+    ``vector_search_agg(..., filter=...)`` restricts a search to the rows matching an MQL predicate over them."""
+
+    def __init__(self, index, name: str = "documents_vectordb_lab2", embedding_column: str = "embedding",
+                 filter_fields=()):
         self.index = index
         self.name = name
         self.embedding_column = embedding_column
+        self.filter_fields = tuple(filter_fields)
+        self.filter_schema = FilterSchema(self.filter_fields) if self.filter_fields else None
         self.document_id: list[str | None] = []
         self.chunk: list[str | None] = []
         self.metadata: list[dict] = []
@@ -141,9 +151,15 @@ class VectorTable:
         # a document repeated inside this very batch: keep its last occurrence only
         last = {d: i for i, d in enumerate(document_ids) if d is not None}
         keep = [i for i, d in enumerate(document_ids) if d is None or last[d] == i]
+        rows = embeddings if len(keep) == n else embeddings[keep]
+        if self.filter_schema is not None:
+            tags = self.filter_schema.tags([metadata[i] for i in keep])   # before anything is mutated: may refuse
         if stale:
             self.index.delete_rows(stale)
-        first = self.index.append(embeddings if len(keep) == n else embeddings[keep])
+        if self.filter_schema is not None:
+            first = self.index.append(rows, tags=tags)
+        else:
+            first = self.index.append(rows)
         assert first == len(self.document_id), "side table and index out of step"
         ids = [document_ids[i] for i in keep]
         chs = [chunks[i] for i in keep]
@@ -165,6 +181,8 @@ class VectorTable:
         shard): row i of the index gets document_ids[i] / chunks[i]."""
         assert len(self.document_id) == 0 and len(document_ids) == len(chunks)
         metadata = metadata or [{} for _ in range(len(document_ids))]
+        if self.filter_schema is not None and len(metadata):
+            self.index.set_tags(np.arange(len(metadata)), self.filter_schema.tags(metadata))
         for d, c, m in zip(document_ids, chunks, metadata):
             if d is not None:
                 self._row_of[d] = len(self.document_id)
@@ -196,7 +214,8 @@ class VectorTable:
             os.fsync(f.fileno())
         os.replace(tmp, os.path.join(directory, files["columns"]))
         man = {"generation": gen, "rows": n, "files": files, "source_offsets": source_offsets or {},
-               "similarity": self.similarity}
+               "similarity": self.similarity, "filter_fields": list(self.filter_fields),
+               "filter_bits": self.filter_schema.to_json()["bits"] if self.filter_schema is not None else []}
         tmp = os.path.join(directory, "manifest.json.tmp")
         with open(tmp, "w") as f:
             json.dump(man, f)
@@ -227,7 +246,9 @@ class VectorTable:
 
     def load(self, directory: str) -> int:
         """Resume from ``save``: restores the index, the side table and ``source_offsets`` (call on an empty table).
-        A checkpoint taken under another similarity is refused (a manifest that does not name one is a cosine one)."""
+        A checkpoint taken under another similarity is refused (a manifest that does not name one is a cosine one), as
+        is one taken with other filter fields; a checkpoint that predates filter fields rebuilds the tags from its
+        metadata column."""
         import json
         import os
         assert len(self) == 0, "load() needs an empty table"
@@ -242,8 +263,15 @@ class VectorTable:
         if saved != self.similarity:
             raise ValueError(f"checkpoint in {directory} was taken with similarity {saved!r}; this table's index uses "
                              f"{self.similarity!r}: rankings and row terms differ, rebuild the table from the log instead")
+        saved_fields = man.get("filter_fields")
+        if saved_fields is not None and tuple(saved_fields) != self.filter_fields:
+            raise ValueError(f"checkpoint in {directory} was taken with filter fields {list(saved_fields)}; this table "
+                             f"declares {list(self.filter_fields)}: rebuild the table from the log instead")
         if len(rows) != man["rows"]:
             raise ValueError(f"snapshot mismatch: manifest says {man['rows']} rows, columns file has {len(rows)}")
+        if self.filter_schema is not None and saved_fields is not None:
+            # the saved bit dictionary: the tags recomputed below are the ones the checkpoint's filters were built on
+            self.filter_schema = FilterSchema.from_json({"fields": saved_fields, "bits": man.get("filter_bits", [])})
         if hasattr(self.index, "restore") and "index" in man["files"]:
             n = self.index.restore(os.path.join(directory, man["files"]["index"]))
             if n != len(rows):
@@ -256,6 +284,8 @@ class VectorTable:
     def clear(self) -> None:
         """What scripts/common/clear_mongodb.py:98-158 does before a re-publish."""
         self.index.reset()
+        if self.filter_schema is not None:
+            self.filter_schema = FilterSchema(self.filter_fields)
         self.document_id.clear()
         self.chunk.clear()
         self.metadata.clear()
@@ -290,9 +320,11 @@ def wire_score_mode(score_mode: str, similarity: str) -> int:
 
 
 def vector_search_agg(table: VectorTable, descriptor: str, query_vectors: np.ndarray, k: int,
-                      score_mode: str = "cosine") -> list[list[SearchHit]]:
+                      score_mode: str = "cosine", filter=None) -> list[list[SearchHit]]:
     """VECTOR_SEARCH_AGG(table, DESCRIPTOR(descriptor), query_vector, k) for a batch of query vectors.
-    ``score_mode``: "cosine" (the raw value of the index's similarity, default) or "atlas" (``atlas_score``)."""
+    ``score_mode``: "cosine" (the raw value of the index's similarity, default) or "atlas" (``atlas_score``).
+    ``filter``: an MQL document over the table's filter fields (``filters.compile_filter``), or a list with one per
+    query; each query's top-k is then the exact top-k of the rows its filter matches."""
     if score_mode not in ("cosine", "atlas"):
         raise ValueError("score_mode must be 'cosine' or 'atlas'")
     if descriptor != table.embedding_column:
@@ -302,7 +334,16 @@ def vector_search_agg(table: VectorTable, descriptor: str, query_vectors: np.nda
         q = q[None, :]
     if q.shape[0] == 0:
         return []
-    score, idx = table.index.search_host(q, k)
+    if filter is None:
+        score, idx = table.index.search_host(q, k)
+    else:
+        if table.filter_schema is None:
+            raise ValueError(f"table {table.name} declares no filter fields")
+        docs = filter if isinstance(filter, (list, tuple)) else [filter] * q.shape[0]
+        if len(docs) != q.shape[0]:
+            raise ValueError(f"{len(docs)} filters for {q.shape[0]} queries")
+        f = np.stack([compile_filter(table.filter_schema, d) for d in docs])
+        score, idx = table.index.search_host(q, k, filters=f)
     out = []
     for r in range(q.shape[0]):
         hits = []

@@ -80,9 +80,10 @@ class ShardedIndex:
         return getattr(self.index, "similarity", "cosine")
 
     # ------------------------------------------------------------------ device-resident queries
-    def search(self, q: torch.Tensor, k: int):
+    def search(self, q: torch.Tensor, k: int, filters=None):
         """q: [nq, dim] bf16 on this rank's device (identical on every rank).  Returns (score f32 [nq,k],
-        global row i64 [nq,k]) -- the same on every rank."""
+        global row i64 [nq,k]) -- the same on every rank.  ``filters`` (uint64 [nq, 4] or [4], the same on every rank)
+        restricts each query to the rows whose tag passes its filter; each rank's index holds its own rows' tags."""
         nq = q.shape[0]
         if self._comm is not None:
             from . import capi
@@ -90,10 +91,19 @@ class ShardedIndex:
             q = q.contiguous()
             score = torch.empty((nq, k), dtype=torch.float32, device=q.device)
             rows = torch.empty((nq, k), dtype=torch.int64, device=q.device)
+            if filters is not None:
+                f = ix._filters_dev(filters, nq, q.device)
+                capi.check(ix.lib.sa_sharded_search_filtered(self._comm, ix._h, q.data_ptr(), f.data_ptr(), nq, k,
+                                                             self.row_offset, score.data_ptr(), rows.data_ptr(),
+                                                             ix._stream()), "sa_sharded_search_filtered")
+                return score, rows
             capi.check(ix.lib.sa_sharded_search(self._comm, ix._h, q.data_ptr(), nq, k, self.row_offset,
                                                 score.data_ptr(), rows.data_ptr(), ix._stream()), "sa_sharded_search")
             return score, rows
-        hits = self.index.search_hits(q, k, self.row_offset)            # uint8 [nq, k, 16]
+        if filters is not None:
+            hits = self.index.search_hits(q, k, self.row_offset, filters=filters)
+        else:
+            hits = self.index.search_hits(q, k, self.row_offset)            # uint8 [nq, k, 16]
         if self.world == 1:
             return self.index.merge_hits(hits.view(1, nq, k, 16))
         key = (nq, k, str(hits.device))
@@ -104,15 +114,22 @@ class ShardedIndex:
         return self.index.merge_hits(gathered.view(self.world, nq, k, 16))
 
     # ------------------------------------------------------------------ host buffers
-    def search_host_submit(self, q_f32: np.ndarray, k: int, slot: int = 0) -> None:
+    def search_host_submit(self, q_f32: np.ndarray, k: int, slot: int = 0, filters=None) -> None:
         """Enqueue H2D + shard scan + all-gather + merge + D2H for ``slot`` (0 or 1) and return at once."""
         q = np.ascontiguousarray(q_f32, dtype=np.float32)
         if self._comm is None:
-            self._inflight[slot] = self._search_host_blocking(q, k)
+            self._inflight[slot] = self._search_host_blocking(q, k, filters)
             return
         from . import capi
+        from .engine import filter_array
         ix = self.index
         self._inflight[slot] = (q, q.shape[0], k)   # keeps a pinned source alive until the wait
+        if filters is not None:
+            f = filter_array(filters, q.shape[0])
+            capi.check(ix.lib.sa_sharded_search_host_submit_filtered(self._comm, ix._h, slot, q.ctypes.data, f.ctypes.data,
+                                                                     q.shape[0], k, self.row_offset),
+                       "sa_sharded_search_host_submit_filtered")
+            return
         capi.check(ix.lib.sa_sharded_search_host_submit(self._comm, ix._h, slot, q.ctypes.data, q.shape[0], k,
                                                         self.row_offset), "sa_sharded_search_host_submit")
 
@@ -130,15 +147,15 @@ class ShardedIndex:
                    "sa_sharded_search_host_wait")
         return score, rows
 
-    def _search_host_blocking(self, q: np.ndarray, k: int):
+    def _search_host_blocking(self, q: np.ndarray, k: int, filters=None):
         dev = self.index.rows.device if hasattr(self.index, "rows") else torch.device("cpu")
         qd = torch.from_numpy(q).to(dev).to(torch.bfloat16)
-        s, gi = self.search(qd, k)
+        s, gi = self.search(qd, k) if filters is None else self.search(qd, k, filters=filters)
         return s.cpu().numpy(), gi.cpu().numpy()
 
-    def search_host(self, q_f32, k: int, out=None):
+    def search_host(self, q_f32, k: int, out=None, filters=None):
         """Host buffers in, host buffers out (H2D, shard search, all-gather, merge, D2H); blocking."""
-        self.search_host_submit(q_f32, k, 0)
+        self.search_host_submit(q_f32, k, 0, filters=filters)
         return self.search_host_wait(0, out=out)
 
 
@@ -196,15 +213,16 @@ class MultiGpuIndex:
         self._where = []
         self._next = 0
 
-    def append(self, rows_f32: np.ndarray) -> int:
-        """Append a batch of fp32 embeddings to the next shard (round-robin).  Returns the first (dense) row id."""
+    def append(self, rows_f32: np.ndarray, tags=None) -> int:
+        """Append a batch of fp32 embeddings to the next shard (round-robin).  Returns the first (dense) row id.
+        ``tags`` (uint64 [n]) are the rows' filter tags (0 without)."""
         rows_f32 = np.ascontiguousarray(rows_f32, dtype=np.float32)
         first = len(self._where)
         if len(rows_f32) == 0:
             return first
         g = self._next
         self._next = (self._next + 1) % self.n
-        lo = self.shards[g].append(rows_f32)
+        lo = self.shards[g].append(rows_f32, tags=tags)
         m = len(rows_f32)
         self._dense_of[g] = np.concatenate([self._dense_of[g], np.arange(first, first + m, dtype=np.int64)])
         self._where.extend((g, lo + j) for j in range(m))
@@ -217,6 +235,18 @@ class MultiGpuIndex:
             by_shard.setdefault(g, []).append(l)
         for g, ls in by_shard.items():
             self.shards[g].delete_rows(ls)
+
+    def set_tags(self, rows, tags) -> None:
+        """Rewrite the filter tags of committed (dense) rows; each shard gets its own rows' tags."""
+        tags = np.ascontiguousarray(tags, dtype=np.uint64)
+        by_shard: dict[int, tuple[list[int], list[int]]] = {}
+        for r, t in zip(rows, tags):
+            g, l = self._where[int(r)]
+            ls, ts = by_shard.setdefault(g, ([], []))
+            ls.append(l)
+            ts.append(t)
+        for g, (ls, ts) in by_shard.items():
+            self.shards[g].set_tags(ls, np.array(ts, dtype=np.uint64))
 
     def _to_dense(self, global_rows: np.ndarray) -> np.ndarray:
         out = np.full(global_rows.shape, -1, dtype=np.int64)
@@ -231,10 +261,18 @@ class MultiGpuIndex:
         out[ok] = dense
         return out
 
-    def search_host_submit(self, q_f32: np.ndarray, k: int, slot: int = 0) -> None:
+    def search_host_submit(self, q_f32: np.ndarray, k: int, slot: int = 0, filters=None) -> None:
+        """``filters`` (uint64 [nq, 4] or [4]) applies to every shard, each filtering its rows by its own tags."""
         from . import capi
+        from .engine import filter_array
         q = np.ascontiguousarray(q_f32, dtype=np.float32)
         self._inflight[slot] = (q, q.shape[0], k)
+        if filters is not None:
+            f = filter_array(filters, q.shape[0])
+            capi.check(self.lib.sa_gather_merge_submit_filtered(self._comm, self._engines, slot, q.ctypes.data,
+                                                                f.ctypes.data, q.shape[0], k, self._offsets),
+                       "sa_gather_merge_submit_filtered")
+            return
         capi.check(self.lib.sa_gather_merge_submit(self._comm, self._engines, slot, q.ctypes.data, q.shape[0], k,
                                                    self._offsets), "sa_gather_merge_submit")
 
@@ -253,6 +291,6 @@ class MultiGpuIndex:
             return out
         return score, dense
 
-    def search_host(self, q_f32: np.ndarray, k: int, out=None):
-        self.search_host_submit(q_f32, k, 0)
+    def search_host(self, q_f32: np.ndarray, k: int, out=None, filters=None):
+        self.search_host_submit(q_f32, k, 0, filters=filters)
         return self.search_host_wait(0, out=out)
