@@ -47,7 +47,9 @@ typedef enum sa_status {
 #define SA_SIM_DOT 1
 #define SA_SIM_EUCLIDEAN 2
 
-#define SA_MAX_K 28 /* candidate lists hold 16 (k <= 16) or 32 entries per tile lane */
+/* Largest k of a search.  Candidate lists hold 16 (k <= 16) or 32 entries per tile lane; a "deep" search (28 < k <= 64)
+ * keeps the 32-entry lists and runs a scan variant whose shared bounds hold for its k (DESIGN.md section 4.1). */
+#define SA_MAX_K 64
 #define SA_HOST_SLOTS 2 /* host-buffer searches that may be in flight at once (sa_search_host_submit) */
 
 int sa_version(void);
@@ -229,9 +231,11 @@ int sa_timing_mean(sa_engine* e, int n, float* scan_ms_mean, float* total_ms_mea
  * drift control between query blocks that share corpus tiles (keeps a shared tile L2-resident so it crosses HBM
  * once): "max_drift" = unpaced lead in tiles (-1 auto), "pace_gain" = delay cycles per K-slice per extra tile
  * of lead (-1 auto, 0 off), "pace_max" = cap of that delay (-1 auto);
- * "share_thresholds" = 1 | 0 (tile lanes exchange per-query top-k thresholds; default 1), "list_len" = 0 (auto) | 16 | 32,
+ * "share_thresholds" = 1 | 0 (tile lanes exchange per-query top-k thresholds; default 1), "list_len" = 0 (auto) | 16 | 32
+ * (16 serves k <= 16, 32 every k <= SA_MAX_K),
  * "window_bound" = 1 | 0 (with >= 16 tile lanes, a lane also bounds its threshold by the (list_len/2)-th largest of 16
- * lanes' second-best scores -- list_len rows in all -- which is far tighter while the lists are young; default 1),
+ * lanes' second-best scores -- list_len rows in all -- which is far tighter while the lists are young; a deep search, k > 28,
+ * takes the 14th largest of their 5th-best scores, 70 rows; default 1),
  * "presample" = S (a pre-pass over every S-th tile seeds those thresholds, so the order of the rows cannot hurt; 0 off, -1 auto),
  * "unit_map" = 0 | 1 (CTA -> (query block, tile lane) mapping), "record_times" = 0 | 1 (per-CTA timestamps),
  * "profile" = 0 | 1 (run the scan's profiling build: per-CTA role wait/busy cycle counters, see sa_scan_profile),
@@ -272,6 +276,9 @@ int sa_debug_list_insert(const float* score, const int32_t* row, int n, int list
  * one query as order-preserving keys, 0 = not published yet) the (list_len/2)-th largest key (0 = no bound yet);
  * out_sorted (optional) receives each window sorted descending by the kernel's 16-input network. */
 int sa_debug_window_bound(const uint32_t* keys, int n_windows, int list_len, uint32_t* out_bound, uint32_t* out_sorted);
+/* The deep search's window bound (28 < k <= 64): for each group of 16 keys (16 tile lanes' 5th-best scores of one query,
+ * 0 = not published yet) the 14th largest key -- 70 rows in all (0 = no bound yet). */
+int sa_debug_window_bound_deep(const uint32_t* keys, int n_windows, uint32_t* out_bound);
 /* The filter predicate (sa_filter) exactly as the scan and the fallback scan evaluate it: out[i] = pass(tags[i], *f). */
 int sa_debug_filter_pass(const uint64_t* tags, int n, const sa_filter* f, uint8_t* out);
 

@@ -17,7 +17,7 @@ SA_ERR_ARG = -2
 SA_ERR_COMM = -3
 SA_ERR_CAPACITY = -4
 SA_ERR_DEVICE = -5
-SA_MAX_K = 28
+SA_MAX_K = 64   # deep searches (28 < k <= 64) keep 32-entry lists with bounds valid for their k
 SA_HOST_SLOTS = 2
 SA_COMM_ID_BYTES = 128
 SA_SIM_COSINE = 0
@@ -44,6 +44,8 @@ EXPORTS = (
     "sa_last_timing", "sa_timing_mean", "sa_set_option",
     "sa_get_info", "sa_scan_profile", "sa_debug_tile_dots", "sa_debug_plan", "sa_debug_float_keys", "sa_debug_bf16_round",
     "sa_debug_merge_keys", "sa_debug_list_insert", "sa_debug_window_bound", "sa_host_alloc", "sa_host_free",
+    # deep search (28 < k <= 64)
+    "sa_debug_window_bound_deep",
     # pre-filtered search
     "sa_corpus_bind_tags", "sa_search_filtered", "sa_search_f32_filtered", "sa_search_host_filtered",
     "sa_search_host_submit_filtered", "sa_search_hits_filtered", "sa_sharded_search_filtered",
@@ -125,6 +127,7 @@ def load() -> C.CDLL:
         "sa_debug_merge_keys": (i32, [vp, vp, i32, vp, vp]),
         "sa_debug_list_insert": (i32, [vp, vp, i32, i32, vp, vp, vp, vp]),
         "sa_debug_window_bound": (i32, [vp, i32, i32, vp, vp]),
+        "sa_debug_window_bound_deep": (i32, [vp, i32, vp]),
         "sa_wire_split_log": (i32, [vp, u64, i32, vp, vp, vp, vp, vp]),
         "sa_wire_decode_queries_embed": (i32, [vp, vp, vp, i32, i32, C.c_uint32, vp, vp, vp, vp, C.POINTER(i32)]),
         "sa_wire_decode_documents_embed": (i32, [vp, vp, vp, i32, i32, C.c_uint32, vp, vp, vp, vp, vp, vp, vp, vp, C.POINTER(i32)]),

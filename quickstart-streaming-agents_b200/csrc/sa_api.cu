@@ -302,6 +302,27 @@ int launch_scan(const CUtensorMap& tq, const CUtensorMap& tc, const sa::ScanPara
 // has the production build only.
 int launch_scan_dispatch(int cg, int kl, int mode, int epi, const CUtensorMap& tq, const CUtensorMap& tc,
                          const sa::ScanParams& p, int grid, cudaStream_t st) {
+  if (epi & sa::kEpiDeep) {  // deep search: 32-entry lists, production build, filtered or not
+    if (mode != sa::kModeProd) return fail(SA_ERR_ARG, "a deep search has no profiling or debug build of the scan");
+    if (kl != 32) return fail(SA_ERR_ARG, "a deep search needs 32-entry candidate lists");
+    constexpr int kD = sa::kEpiDeep;
+    constexpr int kM = sa::kEpiMul | kD, kS = sa::kEpiSub | kD;
+    constexpr int kMF = kM | sa::kEpiFilt, kSF = kS | sa::kEpiFilt;
+    const bool sub = (epi & 1) == sa::kEpiSub, filt = (epi & sa::kEpiFilt) != 0;
+    if (cg == 1) {
+      if (filt) return sub ? launch_scan<1, 32, sa::kModeProd, kSF>(tq, tc, p, grid, st)
+                           : launch_scan<1, 32, sa::kModeProd, kMF>(tq, tc, p, grid, st);
+      return sub ? launch_scan<1, 32, sa::kModeProd, kS>(tq, tc, p, grid, st)
+                 : launch_scan<1, 32, sa::kModeProd, kM>(tq, tc, p, grid, st);
+    }
+    if (cg == 2) {
+      if (filt) return sub ? launch_scan<2, 32, sa::kModeProd, kSF>(tq, tc, p, grid, st)
+                           : launch_scan<2, 32, sa::kModeProd, kMF>(tq, tc, p, grid, st);
+      return sub ? launch_scan<2, 32, sa::kModeProd, kS>(tq, tc, p, grid, st)
+                 : launch_scan<2, 32, sa::kModeProd, kM>(tq, tc, p, grid, st);
+    }
+    return fail(SA_ERR_ARG, "no scan instantiation for cta_group %d list %d", cg, kl);
+  }
   if (epi & sa::kEpiFilt) {
     if (mode != sa::kModeProd) return fail(SA_ERR_ARG, "a filtered search has no profiling or debug build of the scan");
     constexpr int kM = sa::kEpiMul | sa::kEpiFilt, kS = sa::kEpiSub | sa::kEpiFilt;
@@ -402,9 +423,12 @@ int do_search(sa_engine* e, const uint16_t* q_bf16, int nq, int k, float* out_sc
   SA_ON_DEVICE(e->device);
 
   // 16-entry lists for k <= 16: with the certificate any k <= kKL is exact; a margin of spare entries only makes the
-  // fallback rarer, and it is already rare once a tile lane holds more than a few thousand rows
+  // fallback rarer, and it is already rare once a tile lane holds more than a few thousand rows.  A deep search
+  // (k > 28) keeps the 32-entry lists and runs the scan variant whose shared bounds hold for its k (sa_scan.cuh,
+  // kEpiDeep): the certificate needs k <= |U|, not k <= kKL.
   const int kl = e->opt_list_len ? e->opt_list_len : (k <= 16 ? 16 : 32);
-  if (k > kl) return fail(SA_ERR_ARG, "k %d needs candidate lists longer than list_len %d", k, kl);
+  const bool deep = k > sa::kShallowMaxK;
+  if (k > (kl == 32 ? SA_MAX_K : kl)) return fail(SA_ERR_ARG, "k %d needs candidate lists longer than list_len %d", k, kl);
   const int64_t n_rows = e->n_rows;
   const int num_tiles = static_cast<int>((n_rows + sa::kBlockN - 1) / sa::kBlockN);
   const int cg = choose_cg(e, nq);
@@ -412,7 +436,8 @@ int do_search(sa_engine* e, const uint16_t* q_bf16, int nq, int k, float* out_sc
   if (static_cast<int>(plan.size()) > kMaxLaunches)
     return fail(SA_ERR_CAPACITY, "batch needs %zu scan launches (max %d)", plan.size(), kMaxLaunches);
   const int mode = e->opt_profile ? sa::kModeProf : sa::kModeProd;
-  const int epi = (e->sim == SA_SIM_EUCLIDEAN ? sa::kEpiSub : sa::kEpiMul) | (filters != nullptr ? sa::kEpiFilt : 0);
+  const int epi = (e->sim == SA_SIM_EUCLIDEAN ? sa::kEpiSub : sa::kEpiMul) | (filters != nullptr ? sa::kEpiFilt : 0) |
+                  (deep ? sa::kEpiDeep : 0);
   const float eps_rel = scan_eps_rel(e->dim);
 
   // The candidate lists, shared thresholds and drift counters are one set of scratch buffers: a search issued on
@@ -485,7 +510,8 @@ int do_search(sa_engine* e, const uint16_t* q_bf16, int nq, int k, float* out_sc
     SA_CUDA(cudaEventRecord(tm.ev_scan[li][0], st));
     if (do_presample) {
       // Sampling pre-pass: the same kernel over every presample-th tile, then each query's kKL-th best of the sample
-      // becomes its shared threshold (a valid lower bound on its global kKL-th best).  The full scan then starts with
+      // becomes its shared threshold (a valid lower bound on its global kKL-th best; a deep search: its k-th best, a
+      // bound on the global k-th best, and the only seed its shared threshold gets).  The full scan then starts with
       // thresholds near their final values whatever the order of the rows: an adversarial (e.g. ascending) order can no
       // longer make every row an insertion.
       sa::ScanParams pp = sp;
@@ -645,6 +671,8 @@ static_assert(sizeof(sa_filter) == sizeof(sa::Filter) && offsetof(sa_filter, all
                   offsetof(sa_filter, none_of) == offsetof(sa::Filter, none_of) &&
                   offsetof(sa_filter, any_of) == offsetof(sa::Filter, any_of),
               "sa_filter and sa::Filter must share one layout");
+static_assert(SA_MAX_K == sa::kDeepMaxK && sa::kFixMaxK >= SA_MAX_K && sa::kShallowMaxK < SA_MAX_K,
+              "every k <= SA_MAX_K has a scan variant and fits the fallback's lists");
 
 int sa_version(void) { return 100; }
 
@@ -1822,6 +1850,16 @@ int sa_debug_window_bound(const uint32_t* keys, int n_windows, int list_len, uin
     out_bound[w] = list_len == 16 ? sa::window_bound<16>(x) : sa::window_bound<32>(x);
     if (out_sorted)
       for (int i = 0; i < sa::kWin; ++i) out_sorted[static_cast<size_t>(w) * sa::kWin + i] = x[i];
+  }
+  return SA_OK;
+}
+
+int sa_debug_window_bound_deep(const uint32_t* keys, int n_windows, uint32_t* out_bound) {
+  if (!keys || !out_bound || n_windows < 0) return fail(SA_ERR_ARG, "bad argument");
+  for (int w = 0; w < n_windows; ++w) {
+    unsigned x[sa::kWin];
+    for (int i = 0; i < sa::kWin; ++i) x[i] = keys[static_cast<size_t>(w) * sa::kWin + i];
+    out_bound[w] = sa::window_bound<32, true>(x);
   }
   return SA_OK;
 }

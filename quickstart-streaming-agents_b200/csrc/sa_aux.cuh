@@ -259,8 +259,8 @@ struct MergeParams {
   int* fix_count;           // zero at the start of a search
   FixQuery* fix_query;      // [search nq]
   int force_fix;            // test hook: 1 = treat every lane as ambiguous (the fallback then recomputes everything)
-  unsigned* bound_out;      // sampling pre-pass only (else nullptr): publish each query's kKL-th best score of the sample
-                            // into the scan's shared thresholds [nq] and do nothing else
+  unsigned* bound_out;      // sampling pre-pass only (else nullptr): publish each query's max(k, kKL)-th best score of the
+                            // sample into the scan's shared thresholds [nq] and do nothing else
 };
 
 constexpr int kMergeThreads = 160;  // >= kMaxLanes: one thread per tile lane in the head tournament
@@ -393,10 +393,11 @@ __global__ void __launch_bounds__(kMergeThreads) sa_merge_rescore_kernel(const M
   }
   __syncthreads();
 
-  // ---- A_k: k rounds of arg-max over the heads of the (sorted) lane lists; thread t owns lane t
+  // ---- A_k: k rounds of arg-max over the heads of the (sorted) lane lists; thread t owns lane t.  k may exceed kKL (a
+  // deep search): a lane then runs out of entries (cand 0) and the others supply the remaining rounds.
   int head = 0;
   unsigned long long kth = 0;  // key of the k-th best candidate, 0 if fewer than k exist
-  const int rounds = p.bound_out != nullptr ? kKL : p.k;
+  const int rounds = p.bound_out != nullptr ? (p.k > kKL ? p.k : kKL) : p.k;
   for (int round = 0; round < rounds; ++round) {
     const unsigned long long cand = (tid < TL && head < kKL) ? keys[tid * kKL + head] : 0ull;
     unsigned long long wb = cand;
@@ -420,6 +421,8 @@ __global__ void __launch_bounds__(kMergeThreads) sa_merge_rescore_kernel(const M
   if (p.bound_out != nullptr) {
     // Sampling pre-pass: at least kKL rows of the corpus score >= the sample's kKL-th best, so no row scoring less can be
     // in this query's global top-kKL: a valid shared threshold for the full scan that follows (same key as float_to_key).
+    // A deep search (k > kKL) publishes the sample's k-th best over the union instead, a bound on the global k-th best;
+    // a union of fewer than k rows publishes nothing.
     if (tid == 0 && kth != 0ull) atomicMax(p.bound_out + q, static_cast<unsigned>(kth >> 32));
     return;
   }
@@ -539,7 +542,7 @@ struct FixParams {
 
 constexpr int kFixThreads = 256;
 constexpr int kFixChunkTiles = 8;
-constexpr int kFixMaxK = 32;
+constexpr int kFixMaxK = 64;  // per-warp lists of k <= 64 entries in shared memory (SA_MAX_K)
 
 __device__ __forceinline__ void fix_finalize(const FixParams& p, int first, int stride) {
   const int total = p.nq * p.k;

@@ -13,6 +13,8 @@
 // so v is always "larger is better": for euclidean v = <q,c> - |c|^2/2 = (|q|^2 - |q - c|^2) / 2.
 // A filtered search (kEpi | kEpiFilt) also masks, per query, the rows whose 64-bit tag fails the query's Filter: their row
 // term becomes NaN, exactly like a tombstone's, so an ineligible row never enters a list, raises `drop` or a threshold.
+// A deep search (kEpi | kEpiDeep, 28 < k <= 64) keeps the 32-entry lists and changes only the bounds the lanes share
+// (kEpiDeep below).
 //
 // Nothing but the per-CTA candidate lists (kKL entries per query, plus one "dropped" bound per query) leaves the SM.
 //
@@ -59,6 +61,21 @@ constexpr int kModeProf = 2;   // profiling: per-role wait / busy cycle counters
 constexpr int kEpiMul = 0;     // v = acc * w; a row is live iff w > 0 (cosine, dotProduct)
 constexpr int kEpiSub = 1;     // v = acc - w; a row is live iff w >= 0 (euclidean)
 constexpr int kEpiFilt = 2;    // flag: filtered search (ScanParams::row_tags / filters)
+constexpr int kEpiDeep = 4;    // flag: deep search (28 < k <= 64 with kKL = 32 entries): bounds valid for the k-th best
+
+// Deep search.  The list, drop and masking rules are those of every search; only the bounds the lanes share change, since
+// a lane's kKL-th best says nothing about a query's k-th best once k > kKL:
+//   - a lane does not publish its own kKL-th best into thr_shared (it still reads the slot: the deep pre-pass seeds it
+//     with the sample's k-th best, a valid bound for this k);
+//   - the window publishes each lane's kDeepWinPos-th best and takes the kDeepWinRank-th largest of the kWin lanes:
+//     kDeepWinRank lanes with kDeepWinPos rows scoring >= x each are 70 rows >= x, so x never exceeds the k-th best for
+//     any k <= 64 + kDeepMargin (DESIGN.md section 4.1).
+constexpr int kShallowMaxK = 28;  // largest k served by the shallow bounds (32-entry lists, 4 spare entries)
+constexpr int kDeepMaxK = 64;     // = SA_MAX_K
+constexpr int kDeepWinPos = 5;
+constexpr int kDeepWinRank = 14;
+constexpr int kDeepMargin = kDeepWinPos * kDeepWinRank - kDeepMaxK;
+static_assert(kDeepWinRank <= kWin && kDeepMargin >= 6, "the deep window must cover 64 rows plus a margin");
 
 template <int kCG, bool kFilt = false>
 struct ScanCfg {
@@ -111,9 +128,11 @@ struct ScanParams {
   int max_drift;          // lead (in tiles) over the slowest lane-mate that is not paced
   int pace_gain;          // SM cycles of delay per K-slice issue per tile of lead beyond max_drift (0 = free-running)
   int pace_max;           // cap of that delay
-  unsigned* thr_shared;   // [nqb*128*kCG] per-query lower bound on the kKL-th best score, order-preserving keys
-                          // (zero at launch), or nullptr: lanes then learn their thresholds alone
-  unsigned* lane2;        // [tl_count][nqb*128*kCG] each lane's SECOND-best score per query (keys, zero at launch), or
+  unsigned* thr_shared;   // [nqb*128*kCG] per-query lower bound on the kKL-th best score (deep search: on the k-th best,
+                          // seeded by the pre-pass only), order-preserving keys (zero at launch), or nullptr: lanes then
+                          // learn their thresholds alone
+  unsigned* lane2;        // [tl_count][nqb*128*kCG] each lane's SECOND-best score per query (deep search: its
+                          // kDeepWinPos-th best; keys, zero at launch), or
                           // nullptr.  kKL/2 lanes with two rows >= x each are kKL rows >= x: a much tighter bound than
                           // any single lane's kKL-th best while the lists are young (window_bound below)
   long long* dbg_times;   // optional [gridDim.x][2]: globaltimer at CTA start / end (ns), for drift studies
@@ -227,11 +246,13 @@ __host__ __device__ __forceinline__ void sort16_desc(unsigned (&x)[kWin]) {
     }
   }
 }
-template <int kKL>
+// Deep search (kDeep): x[i] is lane i's kDeepWinPos-th best.  If kDeepWinRank different lanes each hold kDeepWinPos rows
+// scoring >= x, 70 rows score >= x: the kDeepWinRank-th largest bounds the k-th best for every k <= 70 (key 0 = no bound).
+template <int kKL, bool kDeep = false>
 __host__ __device__ __forceinline__ unsigned window_bound(unsigned (&x)[kWin]) {
   static_assert(kKL / 2 <= kWin, "the window must hold kKL/2 lanes");
   sort16_desc(x);
-  return x[kKL / 2 - 1];
+  return x[(kDeep ? kDeepWinRank : kKL / 2) - 1];
 }
 
 // One query's candidate list as an epilogue thread holds it: all indices are compile-time, so it lives in registers.
@@ -382,7 +403,10 @@ __global__ void __launch_bounds__(kScanThreads, 1)
 sa_scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_c,
                const ScanParams p) {
   constexpr bool kFilt = (kEpi & kEpiFilt) != 0;
+  constexpr bool kDeep = (kEpi & kEpiDeep) != 0;
+  static_assert(!kDeep || (kKL == 32 && kMode == kModeProd), "deep search: 32-entry lists, production build only");
   using Cfg = ScanCfg<kCG, kFilt>;
+  static_assert(!(kDeep && kFilt) || Cfg::kSmemBytes == 228400, "the filtered deep scan has its twin's smem layout");
   constexpr int kStages = Cfg::kStages;
   constexpr int kRowsPerQb = kBlockM * kCG;
   constexpr bool kProf = (kMode == kModeProf);
@@ -523,7 +547,8 @@ sa_scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant
     // to warm up, and a warp pays for every lane's insertions.  But if ANY lane already holds kKL rows scoring >= x
     // for this query, no row scoring < x can be in the query's global top-kKL.  So each epilogue thread publishes its
     // kKL-th best (atomicMax on an order-preserving key) and reads the shared bound once per tile: every lane gets the
-    // threshold of the whole machine's progress, and the warm-up tail disappears.  The shared bound admits ties (>=),
+    // threshold of the whole machine's progress, and the warm-up tail disappears (a deep search publishes nothing here:
+    // its k-th best may lie past any lane's kKL-th best).  The shared bound admits ties (>=),
     // the thread's own bound stays strict (>), so tie-breaking by row is unchanged.
     const int query = qb * kRowsPerQb + static_cast<int>(rank) * kBlockM + et;
     const bool own_query = epi && query < p.nq;
@@ -588,7 +613,7 @@ sa_scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant
       int slow = 0;
       if (epi) {
         if (have2) {
-          const unsigned kb = window_bound<kKL>(nx2);
+          const unsigned kb = window_bound<kKL, kDeep>(nx2);
           L.nxt_key = kb > L.nxt_key ? kb : L.nxt_key;
           have2 = false;
         }
@@ -714,19 +739,23 @@ sa_scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant
       if constexpr (kProf) slow_chunks += slow;
       if (epi) {
         if (L.slot != nullptr) {
-          if (L.sc[kKL - 1] > L.published) {  // list full and its tail improved: tell the other lanes
-            L.published = L.sc[kKL - 1];
-            atomicMax(L.slot, float_to_key(L.published));
+          // list full and its tail improved: tell the other lanes (a deep search's k-th best may lie past the tail)
+          if constexpr (!kDeep) {
+            if (L.sc[kKL - 1] > L.published) {
+              L.published = L.sc[kKL - 1];
+              atomicMax(L.slot, float_to_key(L.published));
+            }
           }
           L.nxt_key = ld_relaxed_gpu_u32(L.slot);  // consumed at the start of the next tile: latency hidden
         }
-        // publish this lane's second best and, while the lists are young (or whenever a warp just paid for
-        // insertions), fetch the window for the next tile's bound
+        // publish this lane's second best (deep: kDeepWinPos-th best) and, while the lists are young (or whenever a
+        // warp just paid for insertions), fetch the window for the next tile's bound
         if (p.lane2 != nullptr && TL >= kWin) {
           const bool fetch = (ti - tl) / TL < kWinWarmTiles || __any_sync(0xffffffffu, slow > 0);
           if (win_on) {
-            if (L.sc[1] > pub2) {
-              pub2 = L.sc[1];
+            constexpr int kPub = kDeep ? kDeepWinPos - 1 : 1;
+            if (L.sc[kPub] > pub2) {
+              pub2 = L.sc[kPub];
               st_relaxed_gpu_u32(win_q + static_cast<size_t>(tl) * win_stride, float_to_key(pub2));
             }
             if (fetch && ti + TL < walk_tiles) {

@@ -67,6 +67,9 @@ class VectorIndex:
     ordered best first (ascending distance for "euclidean").  ``inv_norm`` holds the row terms: 1/|c| for cosine, 1 for
     dotProduct, |c|^2/2 for euclidean.
 
+    ``max_k`` is the largest k a search may ask for, at most 64 (``capi.SA_MAX_K``); a search with k > 28 runs the deep
+    scan variant and is exact like any other.
+
     ``tags`` holds one 64-bit filter tag per row (uint64 bits in an int64 tensor [capacity]); the searches' ``filters``
     argument restricts each query to the rows whose tag passes its filter (``filter_array``, qsa_b200.filters)."""
 

@@ -321,7 +321,8 @@ def wire_score_mode(score_mode: str, similarity: str) -> int:
 
 def vector_search_agg(table: VectorTable, descriptor: str, query_vectors: np.ndarray, k: int,
                       score_mode: str = "cosine", filter=None) -> list[list[SearchHit]]:
-    """VECTOR_SEARCH_AGG(table, DESCRIPTOR(descriptor), query_vector, k) for a batch of query vectors.
+    """VECTOR_SEARCH_AGG(table, DESCRIPTOR(descriptor), query_vector, k) for a batch of query vectors; k <= the index's
+    max_k (at most 64, Atlas's ``limit``), each query's hits exact and best first.
     ``score_mode``: "cosine" (the raw value of the index's similarity, default) or "atlas" (``atlas_score``).
     ``filter``: an MQL document over the table's filter fields (``filters.compile_filter``), or a list with one per
     query; each query's top-k is then the exact top-k of the rows its filter matches."""

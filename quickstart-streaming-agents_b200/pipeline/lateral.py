@@ -58,7 +58,8 @@ class LateralSearch:
         null, else the embedding of ``query_builder(row)`` / ``row[text_field]``.  ``carry``: upstream columns copied to
         the output (default: all but the vector).  ``query_field``: also emit the query text under this name.
         ``response_field`` + ``prompt_builder`` + ``generator``: append the text generator's answer (ml_predict stub).
-        ``select``: final column list (the outer SELECT), default everything in the order built."""
+        ``select``: final column list (the outer SELECT), default everything in the order built.  ``k`` is at most the
+        index's max_k (up to 64); ``n_out`` (default k) hits per row are projected."""
         if score_mode not in ("cosine", "atlas"):
             raise ValueError("score_mode must be 'cosine' or 'atlas'")
         if text_field is None and query_builder is None and vector_field is None:

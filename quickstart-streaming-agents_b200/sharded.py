@@ -32,6 +32,9 @@ def shard_bounds(n_total: int, world: int, rank: int) -> tuple[int, int]:
 
 
 class ShardedIndex:
+    """One rank's shard (a ``VectorIndex`` made with its own ``max_k``, at most 64) in a torch.distributed job: every rank
+    searches its rows and the per-shard top-k lists are gathered and merged to the global top-k, for any k <= max_k."""
+
     def __init__(self, index, row_offset: int, group=None, transport: str | None = None):
         self.index = index
         self.row_offset = int(row_offset)
@@ -167,7 +170,8 @@ class MultiGpuIndex:
     It offers the interface ``operator.VectorTable`` expects of an index (``append`` -> first row, ``delete_rows``,
     ``reset``, ``__len__``, ``search_host[_submit/_wait]``) with DENSE row ids in append order; inside, append batches go
     round-robin to the shards (SURVEY.md section 8e: "append-only streams go round-robin by epoch") and the library's
-    global rows (shard * capacity + local row) are translated back through a per-shard table."""
+    global rows (shard * capacity + local row) are translated back through a per-shard table.  ``max_k`` (at most 64,
+    ``capi.SA_MAX_K``) is the largest k of a search on every shard."""
 
     def __init__(self, dim: int, capacity_per_gpu: int, max_batch: int, max_k: int, n_gpus: int | None = None,
                  similarity: str = "cosine"):

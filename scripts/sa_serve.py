@@ -27,13 +27,23 @@ except ImportError:
     from _local import resolve_log_dir, setup_logging
 
 
+def _k_arg(v: str) -> int:
+    """VECTOR_SEARCH_AGG k: 1 .. SA_MAX_K (64; searches with k > 28 run the deep scan variant)."""
+    from qsa_b200 import capi    # constants only: loads no library
+    k = int(v)
+    if not 1 <= k <= capi.SA_MAX_K:
+        raise argparse.ArgumentTypeError(f"k must be in [1, {capi.SA_MAX_K}], not {k}")
+    return k
+
+
 def build_parser() -> argparse.ArgumentParser:
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     ap.add_argument("--log-dir", default=None)
     ap.add_argument("--dim", type=int, default=1536)
     ap.add_argument("--capacity", type=int, default=1 << 20, help="rows of HBM to reserve for the vector table (per GPU)")
     ap.add_argument("--max-batch", type=int, default=1024)
-    ap.add_argument("--k", type=int, default=3, help="VECTOR_SEARCH_AGG k (the reference uses 3)")
+    ap.add_argument("--k", type=_k_arg, default=3,
+                    help="VECTOR_SEARCH_AGG k, 1 .. 64 (the reference uses 3; search_results carries the first 3)")
     ap.add_argument("--gpus", type=int, default=1,
                     help="row-shard the table over this many GPUs of the box (one process, NCCL all-gather of the per-shard "
                          "candidates inside libsa_b200.so: sa_comm_create / sa_gather_merge)")
