@@ -11,6 +11,7 @@
 #include <nccl.h>  // types and prototypes only: the library itself is dlopen'ed (sa_comm_*), never linked
 
 #include <algorithm>
+#include <climits>
 #include <cstdarg>
 #include <cstddef>
 #include <cstdio>
@@ -22,10 +23,15 @@ namespace {
 
 thread_local char g_err[512] = "";
 
+int vfail(int rc, const char* fmt, va_list ap) {
+  vsnprintf(g_err, sizeof g_err, fmt, ap);
+  return rc;
+}
+
 int fail(int rc, const char* fmt, ...) {
   va_list ap;
   va_start(ap, fmt);
-  vsnprintf(g_err, sizeof g_err, fmt, ap);
+  vfail(rc, fmt, ap);
   va_end(ap);
   return rc;
 }
@@ -36,7 +42,7 @@ int fail(int rc, const char* fmt, ...) {
 extern "C" int sa_internal_fail(int rc, const char* fmt, ...) {
   va_list ap;
   va_start(ap, fmt);
-  vsnprintf(g_err, sizeof g_err, fmt, ap);
+  vfail(rc, fmt, ap);
   va_end(ap);
   return rc;
 }
@@ -209,7 +215,8 @@ int launch_merge_packed(const sa::PackedHit* hits, int n_shards, int nq, int k, 
     sa::sa_merge_packed_kernel<<<(nq + sa::kMergePackedWarps - 1) / sa::kMergePackedWarps, sa::kMergePackedWarps * 32, 0, st>>>(
         hits, n_shards, nq, k, out_score, out_row, asc);
   else
-    sa::sa_merge_packed_serial_kernel<<<(nq + 127) / 128, 128, 0, st>>>(hits, n_shards, nq, k, out_score, out_row, asc);
+    sa::sa_merge_serial_kernel<<<(nq + 127) / 128, 128, 0, st>>>(sa::PackedHits{hits}, n_shards, nq, k, out_score,
+                                                                  out_row, asc);
   SA_CUDA(cudaGetLastError());
   return SA_OK;
 }
@@ -275,7 +282,7 @@ std::vector<LaunchPlan> plan_search(int num_sms, int max_launch_qblocks, int nq,
   return out;
 }
 
-template <int kCG, int kKL, int kMode, int kEpi = sa::kEpiMul>
+template <int kCG, int kKL, int kMode, int kEpi>
 int launch_scan(const CUtensorMap& tq, const CUtensorMap& tc, const sa::ScanParams& p, int grid, cudaStream_t st) {
   auto kern = sa::sa_scan_kernel<kCG, kKL, kMode, kEpi>;
   constexpr uint32_t kSmem = sa::ScanCfg<kCG, (kEpi & sa::kEpiFilt) != 0>::kSmemBytes;
@@ -297,73 +304,63 @@ int launch_scan(const CUtensorMap& tq, const CUtensorMap& tc, const sa::ScanPara
   return SA_OK;
 }
 
-// epi: sa::kEpiMul (cosine, dotProduct) or sa::kEpiSub (euclidean), | sa::kEpiFilt for a filtered search.  The debug
-// dump reads raw accumulators, which do not depend on the epilogue, so it has the multiply form only; the filtered scan
-// has the production build only.
+// Every instantiation of the scan kernel, one row each: {cta_group, list length, build, epilogue, launcher}.
+// epi: sa::kEpiMul (cosine, dotProduct) or sa::kEpiSub (euclidean), | sa::kEpiFilt for a filtered search,
+// | sa::kEpiDeep for a deep search (k > 28, 32-entry lists).  Filtered and deep searches have the production build
+// only; the profiling build has 16-entry lists only; the debug dump reads raw accumulators, which do not depend on the
+// epilogue, so it has the multiply form only.
+using ScanLauncher = int (*)(const CUtensorMap&, const CUtensorMap&, const sa::ScanParams&, int, cudaStream_t);
+struct ScanVariant {
+  int cg, kl, mode, epi;
+  ScanLauncher launch;
+};
+constexpr int kProd = sa::kModeProd, kProf = sa::kModeProf, kDots = sa::kModeDots;
+constexpr int kMul = sa::kEpiMul, kSub = sa::kEpiSub, kFilt = sa::kEpiFilt, kDeep = sa::kEpiDeep;
+constexpr ScanVariant kScanVariants[] = {
+    // production
+    {1, 16, kProd, kMul, &launch_scan<1, 16, kProd, kMul>},
+    {1, 32, kProd, kMul, &launch_scan<1, 32, kProd, kMul>},
+    {2, 16, kProd, kMul, &launch_scan<2, 16, kProd, kMul>},
+    {2, 32, kProd, kMul, &launch_scan<2, 32, kProd, kMul>},
+    {1, 16, kProd, kSub, &launch_scan<1, 16, kProd, kSub>},
+    {1, 32, kProd, kSub, &launch_scan<1, 32, kProd, kSub>},
+    {2, 16, kProd, kSub, &launch_scan<2, 16, kProd, kSub>},
+    {2, 32, kProd, kSub, &launch_scan<2, 32, kProd, kSub>},
+    {1, 16, kProd, kMul | kFilt, &launch_scan<1, 16, kProd, kMul | kFilt>},
+    {1, 32, kProd, kMul | kFilt, &launch_scan<1, 32, kProd, kMul | kFilt>},
+    {2, 16, kProd, kMul | kFilt, &launch_scan<2, 16, kProd, kMul | kFilt>},
+    {2, 32, kProd, kMul | kFilt, &launch_scan<2, 32, kProd, kMul | kFilt>},
+    {1, 16, kProd, kSub | kFilt, &launch_scan<1, 16, kProd, kSub | kFilt>},
+    {1, 32, kProd, kSub | kFilt, &launch_scan<1, 32, kProd, kSub | kFilt>},
+    {2, 16, kProd, kSub | kFilt, &launch_scan<2, 16, kProd, kSub | kFilt>},
+    {2, 32, kProd, kSub | kFilt, &launch_scan<2, 32, kProd, kSub | kFilt>},
+    // deep
+    {1, 32, kProd, kMul | kDeep, &launch_scan<1, 32, kProd, kMul | kDeep>},
+    {2, 32, kProd, kMul | kDeep, &launch_scan<2, 32, kProd, kMul | kDeep>},
+    {1, 32, kProd, kSub | kDeep, &launch_scan<1, 32, kProd, kSub | kDeep>},
+    {2, 32, kProd, kSub | kDeep, &launch_scan<2, 32, kProd, kSub | kDeep>},
+    {1, 32, kProd, kMul | kFilt | kDeep, &launch_scan<1, 32, kProd, kMul | kFilt | kDeep>},
+    {2, 32, kProd, kMul | kFilt | kDeep, &launch_scan<2, 32, kProd, kMul | kFilt | kDeep>},
+    {1, 32, kProd, kSub | kFilt | kDeep, &launch_scan<1, 32, kProd, kSub | kFilt | kDeep>},
+    {2, 32, kProd, kSub | kFilt | kDeep, &launch_scan<2, 32, kProd, kSub | kFilt | kDeep>},
+    // profiling
+    {1, 16, kProf, kMul, &launch_scan<1, 16, kProf, kMul>},
+    {2, 16, kProf, kMul, &launch_scan<2, 16, kProf, kMul>},
+    {1, 16, kProf, kSub, &launch_scan<1, 16, kProf, kSub>},
+    {2, 16, kProf, kSub, &launch_scan<2, 16, kProf, kSub>},
+    // debug dots
+    {1, 16, kDots, kMul, &launch_scan<1, 16, kDots, kMul>},
+    {2, 16, kDots, kMul, &launch_scan<2, 16, kDots, kMul>},
+};
+
 int launch_scan_dispatch(int cg, int kl, int mode, int epi, const CUtensorMap& tq, const CUtensorMap& tc,
                          const sa::ScanParams& p, int grid, cudaStream_t st) {
-  if (epi & sa::kEpiDeep) {  // deep search: 32-entry lists, production build, filtered or not
-    if (mode != sa::kModeProd) return fail(SA_ERR_ARG, "a deep search has no profiling or debug build of the scan");
-    if (kl != 32) return fail(SA_ERR_ARG, "a deep search needs 32-entry candidate lists");
-    constexpr int kD = sa::kEpiDeep;
-    constexpr int kM = sa::kEpiMul | kD, kS = sa::kEpiSub | kD;
-    constexpr int kMF = kM | sa::kEpiFilt, kSF = kS | sa::kEpiFilt;
-    const bool sub = (epi & 1) == sa::kEpiSub, filt = (epi & sa::kEpiFilt) != 0;
-    if (cg == 1) {
-      if (filt) return sub ? launch_scan<1, 32, sa::kModeProd, kSF>(tq, tc, p, grid, st)
-                           : launch_scan<1, 32, sa::kModeProd, kMF>(tq, tc, p, grid, st);
-      return sub ? launch_scan<1, 32, sa::kModeProd, kS>(tq, tc, p, grid, st)
-                 : launch_scan<1, 32, sa::kModeProd, kM>(tq, tc, p, grid, st);
-    }
-    if (cg == 2) {
-      if (filt) return sub ? launch_scan<2, 32, sa::kModeProd, kSF>(tq, tc, p, grid, st)
-                           : launch_scan<2, 32, sa::kModeProd, kMF>(tq, tc, p, grid, st);
-      return sub ? launch_scan<2, 32, sa::kModeProd, kS>(tq, tc, p, grid, st)
-                 : launch_scan<2, 32, sa::kModeProd, kM>(tq, tc, p, grid, st);
-    }
-    return fail(SA_ERR_ARG, "no scan instantiation for cta_group %d list %d", cg, kl);
-  }
-  if (epi & sa::kEpiFilt) {
-    if (mode != sa::kModeProd) return fail(SA_ERR_ARG, "a filtered search has no profiling or debug build of the scan");
-    constexpr int kM = sa::kEpiMul | sa::kEpiFilt, kS = sa::kEpiSub | sa::kEpiFilt;
-    const bool sub = (epi & 1) == sa::kEpiSub;
-    if (cg == 1 && kl == 16) return sub ? launch_scan<1, 16, sa::kModeProd, kS>(tq, tc, p, grid, st)
-                                        : launch_scan<1, 16, sa::kModeProd, kM>(tq, tc, p, grid, st);
-    if (cg == 1 && kl == 32) return sub ? launch_scan<1, 32, sa::kModeProd, kS>(tq, tc, p, grid, st)
-                                        : launch_scan<1, 32, sa::kModeProd, kM>(tq, tc, p, grid, st);
-    if (cg == 2 && kl == 16) return sub ? launch_scan<2, 16, sa::kModeProd, kS>(tq, tc, p, grid, st)
-                                        : launch_scan<2, 16, sa::kModeProd, kM>(tq, tc, p, grid, st);
-    if (cg == 2 && kl == 32) return sub ? launch_scan<2, 32, sa::kModeProd, kS>(tq, tc, p, grid, st)
-                                        : launch_scan<2, 32, sa::kModeProd, kM>(tq, tc, p, grid, st);
-    return fail(SA_ERR_ARG, "no scan instantiation for cta_group %d list %d", cg, kl);
-  }
-  if (epi == sa::kEpiSub) {
-    if (mode == sa::kModeProf) {
-      if (cg == 1 && kl == 16) return launch_scan<1, 16, sa::kModeProf, sa::kEpiSub>(tq, tc, p, grid, st);
-      if (cg == 2 && kl == 16) return launch_scan<2, 16, sa::kModeProf, sa::kEpiSub>(tq, tc, p, grid, st);
-      return fail(SA_ERR_ARG, "the profiling build of the scan exists for 16-entry lists only");
-    }
-    if (mode != sa::kModeProd) return fail(SA_ERR_ARG, "no euclidean scan instantiation for mode %d", mode);
-    if (cg == 1 && kl == 16) return launch_scan<1, 16, sa::kModeProd, sa::kEpiSub>(tq, tc, p, grid, st);
-    if (cg == 1 && kl == 32) return launch_scan<1, 32, sa::kModeProd, sa::kEpiSub>(tq, tc, p, grid, st);
-    if (cg == 2 && kl == 16) return launch_scan<2, 16, sa::kModeProd, sa::kEpiSub>(tq, tc, p, grid, st);
-    if (cg == 2 && kl == 32) return launch_scan<2, 32, sa::kModeProd, sa::kEpiSub>(tq, tc, p, grid, st);
-    return fail(SA_ERR_ARG, "no scan instantiation for cta_group %d list %d", cg, kl);
-  }
-  if (mode == sa::kModeDots) {
-    if (cg == 1) return launch_scan<1, 16, sa::kModeDots>(tq, tc, p, grid, st);
-    return launch_scan<2, 16, sa::kModeDots>(tq, tc, p, grid, st);
-  }
-  if (mode == sa::kModeProf) {
-    if (cg == 1 && kl == 16) return launch_scan<1, 16, sa::kModeProf>(tq, tc, p, grid, st);
-    if (cg == 2 && kl == 16) return launch_scan<2, 16, sa::kModeProf>(tq, tc, p, grid, st);
-    return fail(SA_ERR_ARG, "the profiling build of the scan exists for 16-entry lists only");
-  }
-  if (cg == 1 && kl == 16) return launch_scan<1, 16, sa::kModeProd>(tq, tc, p, grid, st);
-  if (cg == 1 && kl == 32) return launch_scan<1, 32, sa::kModeProd>(tq, tc, p, grid, st);
-  if (cg == 2 && kl == 16) return launch_scan<2, 16, sa::kModeProd>(tq, tc, p, grid, st);
-  if (cg == 2 && kl == 32) return launch_scan<2, 32, sa::kModeProd>(tq, tc, p, grid, st);
-  return fail(SA_ERR_ARG, "no scan instantiation for cta_group %d list %d", cg, kl);
+  for (const ScanVariant& v : kScanVariants)
+    if (v.cg == cg && v.kl == kl && v.mode == mode && v.epi == epi) return v.launch(tq, tc, p, grid, st);
+  static const char* const kBuild[] = {"production", "debug-dots", "profiling"};  // indexed by sa::kMode*
+  return fail(SA_ERR_ARG, "no scan instantiation for cta_group %d, %d-entry lists, %s build, %s%s%s epilogue", cg, kl,
+              kBuild[mode], (epi & kSub) ? "subtract" : "multiply", (epi & kFilt) ? " filtered" : "",
+              (epi & kDeep) ? " deep" : "");
 }
 
 int choose_cg(const sa_engine* e, int nq) {
@@ -407,6 +404,24 @@ int zero_scan_scratch(sa_engine* e, cudaStream_t st) {
 int check_filtered(const sa_engine* e, const void* filters) {
   if (!filters) return fail(SA_ERR_ARG, "null filters");
   if (!e->row_tags) return fail(SA_ERR_ARG, "filtered search without row tags (call sa_corpus_bind_tags)");
+  return SA_OK;
+}
+
+// The first checks of a search entry point; `filtered`: the filtered twin, which refuses null filters.  The order
+// matters: check_filtered reads the engine, and a sharded search must report an argument error before check_rank_comm,
+// whose first call on a communicator is a collective.
+int check_search(const sa_engine* e, const void* filters, bool filtered) {
+  int rc = check_engine(e);
+  if (rc == SA_OK && filtered) rc = check_filtered(e, filters);
+  return rc;
+}
+
+int convert_queries(sa_engine* e, const float* q_f32_dev, int nq, cudaStream_t st) {
+  SA_CUDA(cudaStreamWaitEvent(st, e->scratch_free, 0));  // q_bf16 is scratch too: the previous search still reads it
+  const long long threads = static_cast<long long>(nq) * 32;
+  sa::sa_convert_rows_kernel<<<static_cast<unsigned>((threads + 255) / 256), 256, 0, st>>>(q_f32_dev, e->q_bf16,
+                                                                                         nullptr, nq, e->dim);
+  SA_CUDA(cudaGetLastError());
   return SA_OK;
 }
 
@@ -507,46 +522,6 @@ int do_search(sa_engine* e, const uint16_t* q_bf16, int nq, int k, float* out_sc
     e->last_grid = grid;
     min_tl = std::min(min_tl, lp.tl);
 
-    SA_CUDA(cudaEventRecord(tm.ev_scan[li][0], st));
-    if (do_presample) {
-      // Sampling pre-pass: the same kernel over every presample-th tile, then each query's kKL-th best of the sample
-      // becomes its shared threshold (a valid lower bound on its global kKL-th best; a deep search: its k-th best, a
-      // bound on the global k-th best, and the only seed its shared threshold gets).  The full scan then starts with
-      // thresholds near their final values whatever the order of the rows: an adversarial (e.g. ascending) order can no
-      // longer make every row an insertion.
-      sa::ScanParams pp = sp;
-      pp.tile_stride = presample;
-      pp.lane_progress = nullptr;  // no pacing: the pre-pass is short
-      pp.pace_gain = 0;
-      pp.lane2 = nullptr;
-      pp.prof = e->prof;
-      rc = launch_scan_dispatch(lp.cg, kl, sa::kModeProd, epi, tq, e->tmap_c[lp.cg - 1], pp, grid, st);
-      if (rc) return rc;
-      sa::MergeParams bp = {};
-      bp.part_score = e->part_score;
-      bp.part_idx = e->part_idx;
-      bp.part_drop = e->part_drop;
-      bp.corpus = e->corpus;
-      bp.queries = qptr;
-      bp.dim = e->dim;
-      bp.nq = lp.nq;
-      bp.k = k;
-      bp.cg = lp.cg;
-      bp.nqb = lp.nqb;
-      bp.tl_count = lp.tl;
-      bp.unit_map = e->opt_unit_map;
-      bp.bound_out = e->thr_shared + lp.q0;
-      if (kl == 16)
-        sa::sa_merge_rescore_kernel<16><<<lp.nq, sa::kMergeThreads, 0, st>>>(bp);
-      else
-        sa::sa_merge_rescore_kernel<32><<<lp.nq, sa::kMergeThreads, 0, st>>>(bp);
-      SA_CUDA(cudaGetLastError());
-      tm.kernels += 2;
-    }
-    rc = launch_scan_dispatch(lp.cg, kl, mode, epi, tq, e->tmap_c[lp.cg - 1], sp, grid, st);
-    if (rc) return rc;
-    SA_CUDA(cudaEventRecord(tm.ev_scan[li][1], st));
-
     sa::MergeParams mp = {};
     mp.part_score = e->part_score;
     mp.part_idx = e->part_idx;
@@ -570,6 +545,34 @@ int do_search(sa_engine* e, const uint16_t* q_bf16, int nq, int k, float* out_sc
     mp.fix_count = e->fix_counters;
     mp.fix_query = e->fix_query;
     mp.force_fix = e->opt_force_fix;
+
+    SA_CUDA(cudaEventRecord(tm.ev_scan[li][0], st));
+    if (do_presample) {
+      // Sampling pre-pass: the same kernel over every presample-th tile, then each query's kKL-th best of the sample
+      // becomes its shared threshold (a valid lower bound on its global kKL-th best; a deep search: its k-th best, a
+      // bound on the global k-th best, and the only seed its shared threshold gets).  The full scan then starts with
+      // thresholds near their final values whatever the order of the rows: an adversarial (e.g. ascending) order can no
+      // longer make every row an insertion.
+      sa::ScanParams pp = sp;
+      pp.tile_stride = presample;
+      pp.lane_progress = nullptr;  // no pacing: the pre-pass is short
+      pp.pace_gain = 0;
+      pp.lane2 = nullptr;
+      pp.prof = e->prof;
+      rc = launch_scan_dispatch(lp.cg, kl, sa::kModeProd, epi, tq, e->tmap_c[lp.cg - 1], pp, grid, st);
+      if (rc) return rc;
+      sa::MergeParams bp = mp;  // with bound_out set the merge kernel publishes the bounds and reads no result field
+      bp.bound_out = e->thr_shared + lp.q0;
+      if (kl == 16)
+        sa::sa_merge_rescore_kernel<16><<<lp.nq, sa::kMergeThreads, 0, st>>>(bp);
+      else
+        sa::sa_merge_rescore_kernel<32><<<lp.nq, sa::kMergeThreads, 0, st>>>(bp);
+      SA_CUDA(cudaGetLastError());
+      tm.kernels += 2;
+    }
+    rc = launch_scan_dispatch(lp.cg, kl, mode, epi, tq, e->tmap_c[lp.cg - 1], sp, grid, st);
+    if (rc) return rc;
+    SA_CUDA(cudaEventRecord(tm.ev_scan[li][1], st));
     if (kl == 16)
       sa::sa_merge_rescore_kernel<16><<<lp.nq, sa::kMergeThreads, 0, st>>>(mp);
     else
@@ -970,45 +973,36 @@ int sa_search(sa_engine* e, const void* q_bf16_dev, int nq, int k, float* out_sc
 
 int sa_search_filtered(sa_engine* e, const void* q_bf16_dev, const sa_filter* filters_dev, int nq, int k,
                        float* out_score_dev, int32_t* out_idx_dev, double* out_score64_dev, uintptr_t stream) {
-  int rc = check_engine(e);
-  if (rc) return rc;
-  rc = check_filtered(e, filters_dev);
+  int rc = check_search(e, filters_dev, true);
   if (rc) return rc;
   return do_search(e, static_cast<const uint16_t*>(q_bf16_dev), nq, k, out_score_dev, out_idx_dev, out_score64_dev,
                    nullptr, 0, reinterpret_cast<cudaStream_t>(stream), reinterpret_cast<const sa::Filter*>(filters_dev));
 }
 
-static int search_f32(sa_engine* e, const float* q_f32_dev, const sa::Filter* filters, int nq, int k,
+static int search_f32(sa_engine* e, const float* q_f32_dev, const sa_filter* filters_dev, bool filtered, int nq, int k,
                       float* out_score_dev, int32_t* out_idx_dev, double* out_score64_dev, uintptr_t stream) {
-  int rc = check_engine(e);
+  int rc = check_search(e, filters_dev, filtered);
   if (rc) return rc;
   if (!q_f32_dev) return fail(SA_ERR_ARG, "null queries");
   if (nq <= 0 || nq > e->max_batch) return fail(SA_ERR_CAPACITY, "nq %d outside [1, max_batch %d]", nq, e->max_batch);
   SA_ON_DEVICE(e->device);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  SA_CUDA(cudaStreamWaitEvent(st, e->scratch_free, 0));  // q_bf16 is scratch too: the previous search still reads it
-  const long long threads = static_cast<long long>(nq) * 32;
-  sa::sa_convert_rows_kernel<<<static_cast<unsigned>((threads + 255) / 256), 256, 0, st>>>(q_f32_dev, e->q_bf16,
-                                                                                         nullptr, nq, e->dim);
-  SA_CUDA(cudaGetLastError());
-  rc = do_search(e, e->q_bf16, nq, k, out_score_dev, out_idx_dev, out_score64_dev, nullptr, 0, st, filters);
+  rc = convert_queries(e, q_f32_dev, nq, st);
+  if (rc) return rc;
+  rc = do_search(e, e->q_bf16, nq, k, out_score_dev, out_idx_dev, out_score64_dev, nullptr, 0, st,
+                 reinterpret_cast<const sa::Filter*>(filters_dev));
   if (rc == SA_OK) e->ring[(e->n_searches - 1) % kTimingRing].kernels += 1;
   return rc;
 }
 
 int sa_search_f32(sa_engine* e, const float* q_f32_dev, int nq, int k, float* out_score_dev, int32_t* out_idx_dev,
                   double* out_score64_dev, uintptr_t stream) {
-  return search_f32(e, q_f32_dev, nullptr, nq, k, out_score_dev, out_idx_dev, out_score64_dev, stream);
+  return search_f32(e, q_f32_dev, nullptr, false, nq, k, out_score_dev, out_idx_dev, out_score64_dev, stream);
 }
 
 int sa_search_f32_filtered(sa_engine* e, const float* q_f32_dev, const sa_filter* filters_dev, int nq, int k,
                            float* out_score_dev, int32_t* out_idx_dev, double* out_score64_dev, uintptr_t stream) {
-  int rc = check_engine(e);
-  if (rc) return rc;
-  rc = check_filtered(e, filters_dev);
-  if (rc) return rc;
-  return search_f32(e, q_f32_dev, reinterpret_cast<const sa::Filter*>(filters_dev), nq, k, out_score_dev, out_idx_dev,
-                    out_score64_dev, stream);
+  return search_f32(e, q_f32_dev, filters_dev, true, nq, k, out_score_dev, out_idx_dev, out_score64_dev, stream);
 }
 
 namespace {
@@ -1137,15 +1131,6 @@ int sharded_search_on_stream(sa_comm* c, int local, sa_engine* e, const uint16_t
   return SA_OK;
 }
 
-int convert_queries(sa_engine* e, const float* q_f32_dev, int nq, cudaStream_t st) {
-  SA_CUDA(cudaStreamWaitEvent(st, e->scratch_free, 0));  // q_bf16 is scratch too: the previous search still reads it
-  const long long threads = static_cast<long long>(nq) * 32;
-  sa::sa_convert_rows_kernel<<<static_cast<unsigned>((threads + 255) / 256), 256, 0, st>>>(q_f32_dev, e->q_bf16, nullptr,
-                                                                                         nq, e->dim);
-  SA_CUDA(cudaGetLastError());
-  return SA_OK;
-}
-
 // Host-buffer search into slot si.  comm == nullptr: this engine alone (shard-local int32 rows); otherwise this rank's
 // part of a sharded search (global int64 rows, identical on every rank).  `phases` as in sharded_search_on_stream
 // (bit 0 also covers the H2D copy and the conversion, bit 2 the D2H copies and the slot's event).  filters_host ([nq],
@@ -1219,22 +1204,9 @@ int host_wait(sa_engine* e, int si, float* out_score_host, void* out_idx_host, b
 
 }  // namespace
 
-int sa_search_host(sa_engine* e, const float* q_f32_host, int nq, int k, float* out_score_host,
-                   int32_t* out_idx_host) {
-  int rc = check_engine(e);
-  if (rc) return rc;
-  if (!out_score_host || !out_idx_host) return fail(SA_ERR_ARG, "null buffer");
-  e->slot[kHostSlots].busy = false;  // the private slot of the blocking call
-  rc = host_submit(e, kHostSlots, q_f32_host, nq, k, nullptr, 0, 0);
-  if (rc) return rc;
-  return host_wait(e, kHostSlots, out_score_host, out_idx_host, false);
-}
-
-int sa_search_host_filtered(sa_engine* e, const float* q_f32_host, const sa_filter* filters_host, int nq, int k,
-                            float* out_score_host, int32_t* out_idx_host) {
-  int rc = check_engine(e);
-  if (rc) return rc;
-  rc = check_filtered(e, filters_host);
+static int search_host(sa_engine* e, const float* q_f32_host, const sa_filter* filters_host, bool filtered, int nq,
+                       int k, float* out_score_host, int32_t* out_idx_host) {
+  int rc = check_search(e, filters_host, filtered);
   if (rc) return rc;
   if (!out_score_host || !out_idx_host) return fail(SA_ERR_ARG, "null buffer");
   e->slot[kHostSlots].busy = false;  // the private slot of the blocking call
@@ -1243,21 +1215,31 @@ int sa_search_host_filtered(sa_engine* e, const float* q_f32_host, const sa_filt
   return host_wait(e, kHostSlots, out_score_host, out_idx_host, false);
 }
 
-int sa_search_host_submit(sa_engine* e, int slot, const float* q_f32_host, int nq, int k) {
-  int rc = check_engine(e);
+int sa_search_host(sa_engine* e, const float* q_f32_host, int nq, int k, float* out_score_host,
+                   int32_t* out_idx_host) {
+  return search_host(e, q_f32_host, nullptr, false, nq, k, out_score_host, out_idx_host);
+}
+
+int sa_search_host_filtered(sa_engine* e, const float* q_f32_host, const sa_filter* filters_host, int nq, int k,
+                            float* out_score_host, int32_t* out_idx_host) {
+  return search_host(e, q_f32_host, filters_host, true, nq, k, out_score_host, out_idx_host);
+}
+
+static int search_host_submit(sa_engine* e, int slot, const float* q_f32_host, const sa_filter* filters_host,
+                              bool filtered, int nq, int k) {
+  int rc = check_search(e, filters_host, filtered);
   if (rc) return rc;
   if (slot < 0 || slot >= kHostSlots) return fail(SA_ERR_ARG, "slot %d outside [0, %d)", slot, kHostSlots);
-  return host_submit(e, slot, q_f32_host, nq, k, nullptr, 0, 0);
+  return host_submit(e, slot, q_f32_host, nq, k, nullptr, 0, 0, 7, filters_host);
+}
+
+int sa_search_host_submit(sa_engine* e, int slot, const float* q_f32_host, int nq, int k) {
+  return search_host_submit(e, slot, q_f32_host, nullptr, false, nq, k);
 }
 
 int sa_search_host_submit_filtered(sa_engine* e, int slot, const float* q_f32_host, const sa_filter* filters_host, int nq,
                                    int k) {
-  int rc = check_engine(e);
-  if (rc) return rc;
-  rc = check_filtered(e, filters_host);
-  if (rc) return rc;
-  if (slot < 0 || slot >= kHostSlots) return fail(SA_ERR_ARG, "slot %d outside [0, %d)", slot, kHostSlots);
-  return host_submit(e, slot, q_f32_host, nq, k, nullptr, 0, 0, 7, filters_host);
+  return search_host_submit(e, slot, q_f32_host, filters_host, true, nq, k);
 }
 
 int sa_search_host_wait(sa_engine* e, int slot, float* out_score_host, int32_t* out_idx_host) {
@@ -1273,32 +1255,16 @@ int sa_merge_shards(sa_engine* e, const double* score64_dev, const int64_t* glob
   if (n_shards <= 0 || n_shards > 64) return fail(SA_ERR_ARG, "n_shards %d outside [1, 64]", n_shards);
   if (nq <= 0 || k <= 0) return fail(SA_ERR_ARG, "nq and k must be positive");
   SA_ON_DEVICE(e->device);
-  sa::sa_merge_shards_kernel<<<(nq + 127) / 128, 128, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      score64_dev, reinterpret_cast<const long long*>(global_idx_dev), n_shards, nq, k, out_score_dev,
+  sa::sa_merge_serial_kernel<<<(nq + 127) / 128, 128, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      sa::SplitHits{score64_dev, reinterpret_cast<const long long*>(global_idx_dev)}, n_shards, nq, k, out_score_dev,
       reinterpret_cast<long long*>(out_idx_dev), e->sim == SA_SIM_EUCLIDEAN);
   SA_CUDA(cudaGetLastError());
   return SA_OK;
 }
 
-int sa_search_hits(sa_engine* e, const void* q_bf16_dev, int nq, int k, int64_t row_offset, sa_hit* out_hits_dev,
-                   uintptr_t stream) {
-  int rc = check_engine(e);
-  if (rc) return rc;
-  if (!out_hits_dev) return fail(SA_ERR_ARG, "null buffer");
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  {
-    SA_ON_DEVICE(e->device);
-    SA_CUDA(cudaStreamWaitEvent(st, e->scratch_free, 0));  // res_score / res_idx below are engine scratch
-  }
-  return do_search(e, static_cast<const uint16_t*>(q_bf16_dev), nq, k, e->res_score, e->res_idx, nullptr,
-                   reinterpret_cast<sa::PackedHit*>(out_hits_dev), row_offset, st);
-}
-
-int sa_search_hits_filtered(sa_engine* e, const void* q_bf16_dev, const sa_filter* filters_dev, int nq, int k,
-                            int64_t row_offset, sa_hit* out_hits_dev, uintptr_t stream) {
-  int rc = check_engine(e);
-  if (rc) return rc;
-  rc = check_filtered(e, filters_dev);
+static int search_hits(sa_engine* e, const void* q_bf16_dev, const sa_filter* filters_dev, bool filtered, int nq, int k,
+                       int64_t row_offset, sa_hit* out_hits_dev, uintptr_t stream) {
+  int rc = check_search(e, filters_dev, filtered);
   if (rc) return rc;
   if (!out_hits_dev) return fail(SA_ERR_ARG, "null buffer");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
@@ -1309,6 +1275,16 @@ int sa_search_hits_filtered(sa_engine* e, const void* q_bf16_dev, const sa_filte
   return do_search(e, static_cast<const uint16_t*>(q_bf16_dev), nq, k, e->res_score, e->res_idx, nullptr,
                    reinterpret_cast<sa::PackedHit*>(out_hits_dev), row_offset, st,
                    reinterpret_cast<const sa::Filter*>(filters_dev));
+}
+
+int sa_search_hits(sa_engine* e, const void* q_bf16_dev, int nq, int k, int64_t row_offset, sa_hit* out_hits_dev,
+                   uintptr_t stream) {
+  return search_hits(e, q_bf16_dev, nullptr, false, nq, k, row_offset, out_hits_dev, stream);
+}
+
+int sa_search_hits_filtered(sa_engine* e, const void* q_bf16_dev, const sa_filter* filters_dev, int nq, int k,
+                            int64_t row_offset, sa_hit* out_hits_dev, uintptr_t stream) {
+  return search_hits(e, q_bf16_dev, filters_dev, true, nq, k, row_offset, out_hits_dev, stream);
 }
 
 int sa_merge_hits(sa_engine* e, const sa_hit* hits_dev, int n_shards, int nq, int k, float* out_score_dev,
@@ -1437,25 +1413,10 @@ int check_rank_comm(sa_comm* c, const sa_engine* e) {
 }
 }  // namespace
 
-int sa_sharded_search(sa_comm* c, sa_engine* e, const void* q_bf16_dev, int nq, int k, int64_t row_offset,
-                      float* out_score_dev, int64_t* out_row_dev, uintptr_t stream) {
-  int rc = check_engine(e);
-  if (rc) return rc;
-  rc = check_rank_comm(c, e);
-  if (rc) return rc;
-  if (!out_score_dev || !out_row_dev) return fail(SA_ERR_ARG, "null buffer");
-  SA_ON_DEVICE(e->device);
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  SA_CUDA(cudaStreamWaitEvent(st, e->scratch_free, 0));
-  return sharded_search_on_stream(c, 0, e, static_cast<const uint16_t*>(q_bf16_dev), nq, k, row_offset, out_score_dev,
-                                  reinterpret_cast<long long*>(out_row_dev), st);
-}
-
-int sa_sharded_search_filtered(sa_comm* c, sa_engine* e, const void* q_bf16_dev, const sa_filter* filters_dev, int nq,
-                               int k, int64_t row_offset, float* out_score_dev, int64_t* out_row_dev, uintptr_t stream) {
-  int rc = check_engine(e);
-  if (rc) return rc;
-  rc = check_filtered(e, filters_dev);
+static int sharded_search(sa_comm* c, sa_engine* e, const void* q_bf16_dev, const sa_filter* filters_dev, bool filtered,
+                          int nq, int k, int64_t row_offset, float* out_score_dev, int64_t* out_row_dev,
+                          uintptr_t stream) {
+  int rc = check_search(e, filters_dev, filtered);
   if (rc) return rc;
   rc = check_rank_comm(c, e);
   if (rc) return rc;
@@ -1468,26 +1429,34 @@ int sa_sharded_search_filtered(sa_comm* c, sa_engine* e, const void* q_bf16_dev,
                                   reinterpret_cast<const sa::Filter*>(filters_dev));
 }
 
-int sa_sharded_search_host_submit(sa_comm* c, sa_engine* e, int slot, const float* q_f32_host, int nq, int k,
-                                  int64_t row_offset) {
-  int rc = check_engine(e);
-  if (rc) return rc;
-  rc = check_rank_comm(c, e);
-  if (rc) return rc;
-  if (slot < 0 || slot >= kHostSlots) return fail(SA_ERR_ARG, "slot %d outside [0, %d)", slot, kHostSlots);
-  return host_submit(e, slot, q_f32_host, nq, k, c, 0, row_offset);
+int sa_sharded_search(sa_comm* c, sa_engine* e, const void* q_bf16_dev, int nq, int k, int64_t row_offset,
+                      float* out_score_dev, int64_t* out_row_dev, uintptr_t stream) {
+  return sharded_search(c, e, q_bf16_dev, nullptr, false, nq, k, row_offset, out_score_dev, out_row_dev, stream);
 }
 
-int sa_sharded_search_host_submit_filtered(sa_comm* c, sa_engine* e, int slot, const float* q_f32_host,
-                                           const sa_filter* filters_host, int nq, int k, int64_t row_offset) {
-  int rc = check_engine(e);
-  if (rc) return rc;
-  rc = check_filtered(e, filters_host);
+int sa_sharded_search_filtered(sa_comm* c, sa_engine* e, const void* q_bf16_dev, const sa_filter* filters_dev, int nq,
+                               int k, int64_t row_offset, float* out_score_dev, int64_t* out_row_dev, uintptr_t stream) {
+  return sharded_search(c, e, q_bf16_dev, filters_dev, true, nq, k, row_offset, out_score_dev, out_row_dev, stream);
+}
+
+static int sharded_search_host_submit(sa_comm* c, sa_engine* e, int slot, const float* q_f32_host,
+                                      const sa_filter* filters_host, bool filtered, int nq, int k, int64_t row_offset) {
+  int rc = check_search(e, filters_host, filtered);
   if (rc) return rc;
   rc = check_rank_comm(c, e);
   if (rc) return rc;
   if (slot < 0 || slot >= kHostSlots) return fail(SA_ERR_ARG, "slot %d outside [0, %d)", slot, kHostSlots);
   return host_submit(e, slot, q_f32_host, nq, k, c, 0, row_offset, 7, filters_host);
+}
+
+int sa_sharded_search_host_submit(sa_comm* c, sa_engine* e, int slot, const float* q_f32_host, int nq, int k,
+                                  int64_t row_offset) {
+  return sharded_search_host_submit(c, e, slot, q_f32_host, nullptr, false, nq, k, row_offset);
+}
+
+int sa_sharded_search_host_submit_filtered(sa_comm* c, sa_engine* e, int slot, const float* q_f32_host,
+                                           const sa_filter* filters_host, int nq, int k, int64_t row_offset) {
+  return sharded_search_host_submit(c, e, slot, q_f32_host, filters_host, true, nq, k, row_offset);
 }
 
 int sa_sharded_search_host_wait(sa_comm* c, sa_engine* e, int slot, float* out_score_host, int64_t* out_row_host) {
@@ -1635,75 +1604,51 @@ int sa_timing_mean(sa_engine* e, int n, float* scan_ms_mean, float* total_ms_mea
   return SA_OK;
 }
 
+namespace {
+// Options of sa_set_option: the engine field each sets and the values it accepts.  A flag accepts any value and stores
+// 1 for a nonzero one; any other option accepts [lo, hi].
+using EngineField = int sa_engine::*;
+struct EngineOption {
+  const char* name;
+  EngineField field;
+  bool flag;
+  int64_t lo = 0, hi = 0;
+};
+constexpr EngineOption kOptions[] = {
+    {"cta_group", &sa_engine::opt_cta_group, false, 0, 2},
+    {"unit_map", &sa_engine::opt_unit_map, false, 0, 1},
+    {"wait_hint_ns", &sa_engine::opt_wait_hint_ns, false, -1, 1000000},
+    {"presample", &sa_engine::opt_presample, false, -1, 4096},
+    {"pace_gain", &sa_engine::opt_pace_gain, false, -1, 4096},
+    {"pace_max", &sa_engine::opt_pace_max, false, -1, 65536},
+    {"max_drift", &sa_engine::opt_max_drift, false, -1, 1024},
+    {"max_launch_qblocks", &sa_engine::opt_max_launch_qblocks, false, 0, INT_MAX},
+    {"force_fix", &sa_engine::opt_force_fix, true},
+    {"count_fix", &sa_engine::opt_count_fix, true},
+    {"profile", &sa_engine::opt_profile, true},
+    {"share_thresholds", &sa_engine::opt_share_thresholds, true},
+    {"window_bound", &sa_engine::opt_window_bound, true},
+    {"record_times", &sa_engine::opt_record_times, true},
+};
+}  // namespace
+
 int sa_set_option(sa_engine* e, const char* name, int64_t value) {
   if (!e || !name) return fail(SA_ERR_ARG, "null argument");
-  if (!strcmp(name, "cta_group")) {
-    if (value < 0 || value > 2) return fail(SA_ERR_ARG, "cta_group must be 0, 1 or 2");
-    e->opt_cta_group = static_cast<int>(value);
-    return SA_OK;
-  }
-  if (!strcmp(name, "max_launch_qblocks")) {
-    if (value < 0) return fail(SA_ERR_ARG, "max_launch_qblocks must be >= 0");
-    e->opt_max_launch_qblocks = static_cast<int>(value);
-    return SA_OK;
-  }
-  if (!strcmp(name, "wait_hint_ns")) {
-    if (value < -1 || value > 1000000) return fail(SA_ERR_ARG, "wait_hint_ns must be in [-1, 1000000]");
-    e->opt_wait_hint_ns = static_cast<int>(value);
-    return SA_OK;
-  }
-  if (!strcmp(name, "presample")) {
-    if (value < -1 || value > 4096) return fail(SA_ERR_ARG, "presample must be in [-1, 4096]");
-    e->opt_presample = static_cast<int>(value);
-    return SA_OK;
-  }
-  if (!strcmp(name, "force_fix")) {
-    e->opt_force_fix = value ? 1 : 0;
-    return SA_OK;
-  }
-  if (!strcmp(name, "count_fix")) {
-    e->opt_count_fix = value ? 1 : 0;
-    return SA_OK;
-  }
-  if (!strcmp(name, "profile")) {
-    e->opt_profile = value ? 1 : 0;
-    return SA_OK;
-  }
-  if (!strcmp(name, "share_thresholds")) {
-    e->opt_share_thresholds = value ? 1 : 0;
-    return SA_OK;
-  }
-  if (!strcmp(name, "window_bound")) {
-    e->opt_window_bound = value ? 1 : 0;
-    return SA_OK;
-  }
-  if (!strcmp(name, "list_len")) {
+  if (!strcmp(name, "list_len")) {  // the one option whose values are a set rather than a range
     if (value != 0 && value != 16 && value != 32) return fail(SA_ERR_ARG, "list_len must be 0, 16 or 32");
     e->opt_list_len = static_cast<int>(value);
     return SA_OK;
   }
-  if (!strcmp(name, "record_times")) {
-    e->opt_record_times = value ? 1 : 0;
-    return SA_OK;
-  }
-  if (!strcmp(name, "unit_map")) {
-    if (value < 0 || value > 1) return fail(SA_ERR_ARG, "unit_map must be 0 or 1");
-    e->opt_unit_map = static_cast<int>(value);
-    return SA_OK;
-  }
-  if (!strcmp(name, "pace_gain")) {
-    if (value < -1 || value > 4096) return fail(SA_ERR_ARG, "pace_gain must be in [-1, 4096]");
-    e->opt_pace_gain = static_cast<int>(value);
-    return SA_OK;
-  }
-  if (!strcmp(name, "pace_max")) {
-    if (value < -1 || value > 65536) return fail(SA_ERR_ARG, "pace_max must be in [-1, 65536]");
-    e->opt_pace_max = static_cast<int>(value);
-    return SA_OK;
-  }
-  if (!strcmp(name, "max_drift")) {
-    if (value < -1 || value > 1024) return fail(SA_ERR_ARG, "max_drift must be in [-1, 1024]");
-    e->opt_max_drift = static_cast<int>(value);
+  for (const EngineOption& o : kOptions) {
+    if (strcmp(name, o.name)) continue;
+    if (o.flag) {
+      e->*o.field = value != 0;
+      return SA_OK;
+    }
+    if (value < o.lo || value > o.hi)
+      return fail(SA_ERR_ARG, "%s must be in [%lld, %lld]", name, static_cast<long long>(o.lo),
+                  static_cast<long long>(o.hi));
+    e->*o.field = static_cast<int>(value);
     return SA_OK;
   }
   return fail(SA_ERR_ARG, "unknown option '%s'", name);
@@ -1771,15 +1716,7 @@ int sa_debug_tile_dots(sa_engine* e, const void* q_bf16_dev, int nq, int tile, i
   sp.part_score = e->part_score;
   sp.part_idx = e->part_idx;
   sp.part_drop = e->part_drop;
-  sp.corpus_evict_first = 0;
   sp.tile_stride = 1;
-  sp.lane_progress = nullptr;
-  sp.max_drift = 0;
-  sp.pace_gain = 0;
-  sp.pace_max = 0;
-  sp.unit_map = 0;
-  sp.thr_shared = nullptr;
-  sp.dbg_times = nullptr;
   sp.dbg_dots = out_dots_dev;
   sp.dbg_tile = tile;
   return launch_scan_dispatch(cta_group, 16, sa::kModeDots, sa::kEpiMul, tq, e->tmap_c[cta_group - 1], sp, nqb * cta_group,

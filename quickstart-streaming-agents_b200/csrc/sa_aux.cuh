@@ -8,16 +8,18 @@
 
 namespace sa {
 
-__host__ __device__ __forceinline__ uint32_t aux_f32_bits(float f) {
+// Bit casts usable on both sides of the compiler: the device path is the intrinsic, the host path (used only by the
+// CPU unit tests through sa_debug_*) is a memcpy.
+__host__ __device__ __forceinline__ unsigned f32_bits(float f) {
 #ifdef __CUDA_ARCH__
   return __float_as_uint(f);
 #else
-  uint32_t u;
+  unsigned u;
   memcpy(&u, &f, sizeof u);
   return u;
 #endif
 }
-__host__ __device__ __forceinline__ float aux_bits_f32(uint32_t u) {
+__host__ __device__ __forceinline__ float bits_f32(unsigned u) {
 #ifdef __CUDA_ARCH__
   return __uint_as_float(u);
 #else
@@ -26,10 +28,21 @@ __host__ __device__ __forceinline__ float aux_bits_f32(uint32_t u) {
   return f;
 #endif
 }
-__host__ __device__ __forceinline__ float bf16_bits_to_f32(uint32_t b) { return aux_bits_f32(b << 16); }
+
+// Order-preserving float <-> unsigned key (larger float <=> larger key; key 0 is below every float).  The scan's shared
+// thresholds hold these keys, and the merge kernel's 64-bit keys (make_key) carry one in their high word.
+__host__ __device__ __forceinline__ unsigned float_to_key(float f) {
+  const unsigned u = f32_bits(f);
+  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+__host__ __device__ __forceinline__ float key_to_float(unsigned k) {
+  return bits_f32((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
+}
+
+__host__ __device__ __forceinline__ float bf16_bits_to_f32(uint32_t b) { return bits_f32(b << 16); }
 // Round-to-nearest-even fp32 -> bf16 bit pattern (NaN kept quiet); same rule as the oracle's numpy code.
 __host__ __device__ __forceinline__ uint32_t f32_to_bf16_bits(float f) {
-  uint32_t u = aux_f32_bits(f);
+  uint32_t u = f32_bits(f);
   if ((u & 0x7fffffffu) > 0x7f800000u) return (u >> 16) | 0x40u;
   return (u + 0x7fffu + ((u >> 16) & 1u)) >> 16;
 }
@@ -201,11 +214,9 @@ __host__ __device__ __forceinline__ bool filter_pass(unsigned long long t, const
          ((f.any_of[1] == 0ull) | ((t & f.any_of[1]) != 0ull));
 }
 
-// Order-preserving map: (score desc, row asc)  <=>  key desc.
+// Order-preserving map: (score desc, row asc)  <=>  key desc.  The high word is float_to_key(score).
 __host__ __device__ __forceinline__ unsigned long long make_key(float s, int row) {
-  uint32_t u = aux_f32_bits(s);
-  u = (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-  return (static_cast<unsigned long long>(u) << 32) | static_cast<uint32_t>(~static_cast<uint32_t>(row));
+  return (static_cast<unsigned long long>(float_to_key(s)) << 32) | static_cast<uint32_t>(~static_cast<uint32_t>(row));
 }
 __host__ __device__ __forceinline__ int key_row(unsigned long long k) { return static_cast<int>(~static_cast<uint32_t>(k)); }
 
@@ -269,8 +280,7 @@ constexpr int kMaxLanes = 132;      // tile lanes of one scan launch (the planne
 constexpr int kSelMax = 128;        // candidates re-scored per query without the fallback
 
 __device__ __forceinline__ float key_score(unsigned long long k) {
-  const uint32_t u = static_cast<uint32_t>(k >> 32);
-  return aux_bits_f32((u & 0x80000000u) ? (u & 0x7fffffffu) : ~u);
+  return key_to_float(static_cast<unsigned>(k >> 32));
 }
 
 // Exact internal value of (query, corpus row), one warp: bf16 x bf16 products are exact in fp32; sums of products and of
@@ -420,7 +430,8 @@ __global__ void __launch_bounds__(kMergeThreads) sa_merge_rescore_kernel(const M
   }
   if (p.bound_out != nullptr) {
     // Sampling pre-pass: at least kKL rows of the corpus score >= the sample's kKL-th best, so no row scoring less can be
-    // in this query's global top-kKL: a valid shared threshold for the full scan that follows (same key as float_to_key).
+    // in this query's global top-kKL: a valid shared threshold for the full scan that follows (kth >> 32 is the score's
+    // float_to_key, the scan's own key: see make_key).
     // A deep search (k > kKL) publishes the sample's k-th best over the union instead, a bound on the global k-th best;
     // a union of fewer than k rows publishes nothing.
     if (tid == 0 && kth != 0ull) atomicMax(p.bound_out + q, static_cast<unsigned>(kth >> 32));
@@ -758,47 +769,20 @@ sa_merge_packed_kernel(const PackedHit* __restrict__ hits, int n_shards, int nq,
   }
 }
 
-// The same merge for any number of shards (one thread per query); used when n_shards > 32 or n_shards * k > 256.
-__global__ void sa_merge_packed_serial_kernel(const PackedHit* __restrict__ hits, int n_shards, int nq, int k,
-                                              float* __restrict__ out_score, long long* __restrict__ out_idx, int asc) {
-  const int q = blockIdx.x * blockDim.x + threadIdx.x;
-  if (q >= nq) return;
-  int head[64];
-  for (int g = 0; g < n_shards; ++g) head[g] = 0;
-  for (int i = 0; i < k; ++i) {
-    int bg = -1;
-    double bs = 0.0;
-    long long bi = 0;
-    for (int g = 0; g < n_shards; ++g) {
-      if (head[g] >= k) continue;
-      const PackedHit h = hits[(static_cast<size_t>(g) * nq + q) * k + head[g]];
-      if (h.row < 0) {
-        head[g] = k;
-        continue;
-      }
-      const double hs = asc ? -h.score : h.score;
-      if (bg < 0 || hs > bs || (hs == bs && h.row < bi)) {
-        bg = g;
-        bs = hs;
-        bi = h.row;
-      }
-    }
-    const size_t oo = static_cast<size_t>(q) * k + i;
-    if (bg >= 0) {
-      out_score[oo] = static_cast<float>(asc ? -bs : bs);
-      out_idx[oo] = bi;
-      ++head[bg];
-    } else {
-      out_score[oo] = asc ? INFINITY : -INFINITY;
-      out_idx[oo] = -1;
-    }
-  }
-}
-
-// After the all-gather: per query, merge G shard lists of k (already sorted, global row ids) into the
-// global top-k by (value desc, global row asc), or (value asc, ...) when asc.  One thread per query; G*k <= a few hundred.
-__global__ void sa_merge_shards_kernel(const double* __restrict__ score64, const long long* __restrict__ gidx,
-                                       int n_shards, int nq, int k, float* __restrict__ out_score,
+// The same merge for any number of shards (<= 64), one thread per query: the fallback of sa_merge_packed_kernel when
+// n_shards > 32, k > 32 or n_shards * k > 256, and the merge of sa_merge_shards.  `Hits` loads hit o of the
+// [n_shards][nq][k] lists: packed sa_hit records (PackedHits) or separate score and row arrays (SplitHits).
+struct PackedHits {
+  const PackedHit* __restrict__ hits;
+  __device__ __forceinline__ PackedHit at(size_t o) const { return hits[o]; }
+};
+struct SplitHits {
+  const double* __restrict__ score;
+  const long long* __restrict__ row;
+  __device__ __forceinline__ PackedHit at(size_t o) const { return PackedHit{score[o], row[o]}; }
+};
+template <typename Hits>
+__global__ void sa_merge_serial_kernel(const Hits hits, int n_shards, int nq, int k, float* __restrict__ out_score,
                                        long long* __restrict__ out_idx, int asc) {
   const int q = blockIdx.x * blockDim.x + threadIdx.x;
   if (q >= nq) return;
@@ -810,17 +794,16 @@ __global__ void sa_merge_shards_kernel(const double* __restrict__ score64, const
     long long bi = 0;
     for (int g = 0; g < n_shards; ++g) {
       if (head[g] >= k) continue;
-      const size_t o = (static_cast<size_t>(g) * nq + q) * k + head[g];
-      const long long ri = gidx[o];
-      if (ri < 0) {
+      const PackedHit h = hits.at((static_cast<size_t>(g) * nq + q) * k + head[g]);
+      if (h.row < 0) {
         head[g] = k;
         continue;
       }
-      const double s = asc ? -score64[o] : score64[o];
-      if (bg < 0 || s > bs || (s == bs && ri < bi)) {
+      const double hs = asc ? -h.score : h.score;
+      if (bg < 0 || hs > bs || (hs == bs && h.row < bi)) {
         bg = g;
-        bs = s;
-        bi = ri;
+        bs = hs;
+        bi = h.row;
       }
     }
     const size_t oo = static_cast<size_t>(q) * k + i;

@@ -34,7 +34,6 @@
 #include "sa_aux.cuh"
 #include "sm90_ptx.cuh"
 #include <cmath>
-#include <cstring>
 
 namespace sa {
 
@@ -143,35 +142,6 @@ struct ScanParams {
   const Filter* filters;               // kEpiFilt only: [nq] this launch's queries' filters
 };
 
-// Bit casts usable on both sides of the compiler: the device path is the intrinsic, the host path (used only by the
-// CPU unit tests through sa_debug_*) is a memcpy.
-__host__ __device__ __forceinline__ unsigned f32_bits(float f) {
-#ifdef __CUDA_ARCH__
-  return __float_as_uint(f);
-#else
-  unsigned u;
-  memcpy(&u, &f, sizeof u);
-  return u;
-#endif
-}
-__host__ __device__ __forceinline__ float bits_f32(unsigned u) {
-#ifdef __CUDA_ARCH__
-  return __uint_as_float(u);
-#else
-  float f;
-  memcpy(&f, &u, sizeof f);
-  return f;
-#endif
-}
-
-// Order-preserving float <-> unsigned key (larger float <=> larger key; key 0 is below every float).
-__host__ __device__ __forceinline__ unsigned float_to_key(float f) {
-  const unsigned u = f32_bits(f);
-  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-__host__ __device__ __forceinline__ float key_to_float(unsigned k) {
-  return bits_f32((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
-}
 // The largest float strictly less than x (x finite): `s > float_below(x)` <=> `s >= x`.
 __host__ __device__ __forceinline__ float float_below(float x) {
   const int b = static_cast<int>(f32_bits(x));

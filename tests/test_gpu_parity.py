@@ -538,9 +538,33 @@ def test_c_abi_error_behaviour_on_device(bf):
     assert lib.sa_engine_create(C.byref(unbound), 0, 128, 1000, 64, 10) == 0
     assert lib.sa_search(unbound, q.data_ptr(), 8, 5, s.data_ptr(), i.data_ptr(), None, st) == capi.SA_ERR_ARG
     assert b"sa_corpus_bind" in lib.sa_last_error()
+    # every option takes both ends of its range and refuses one past each; a flag takes any value
+    for name, lo, hi in (("cta_group", 0, 2), ("unit_map", 0, 1), ("wait_hint_ns", -1, 1_000_000),
+                         ("presample", -1, 4096), ("pace_gain", -1, 4096), ("pace_max", -1, 65536),
+                         ("max_drift", -1, 1024), ("max_launch_qblocks", 0, 2**31 - 1)):
+        for v, rc in ((lo - 1, capi.SA_ERR_ARG), (lo, 0), (hi, 0), (hi + 1, capi.SA_ERR_ARG)):
+            assert lib.sa_set_option(unbound, name.encode(), v) == rc, (name, v)
+    assert lib.sa_set_option(unbound, b"max_launch_qblocks", 2**32) == capi.SA_ERR_ARG   # not wrapped to 0 ("no cap")
+    for v, rc in ((0, 0), (16, 0), (32, 0), (-1, capi.SA_ERR_ARG), (15, capi.SA_ERR_ARG), (33, capi.SA_ERR_ARG)):
+        assert lib.sa_set_option(unbound, b"list_len", v) == rc, ("list_len", v)
+    for name in ("force_fix", "count_fix", "profile", "share_thresholds", "window_bound", "record_times"):
+        for v in (0, 1, 7):
+            assert lib.sa_set_option(unbound, name.encode(), v) == 0, (name, v)
     lib.sa_engine_destroy(unbound)
     check(ix, bf.synth_rows(2, 0, 64, 128), c, 10)                        # still healthy after all of that
     ix.close()
+    # the profiling build of the scan has 16-entry lists only and no filtered or deep form: such searches are refused,
+    # and the engine answers exactly once the option is off again
+    deep = VectorIndex(dim=128, capacity=1000, max_batch=64, max_k=capi.SA_MAX_K)
+    deep.append_bf16_bits(c)
+    deep.set_option("profile", 1)
+    for k, filters in ((20, None), (10, np.zeros(4, np.uint64)), (29, None)):
+        with pytest.raises(capi.SaError) as err:
+            deep.search(q, k, filters=filters)
+        assert err.value.rc == capi.SA_ERR_ARG, (k, filters)
+    deep.set_option("profile", 0)
+    check(deep, bf.synth_rows(2, 0, 64, 128), c, 10)
+    deep.close()
 
 
 @pytest.mark.parametrize("cg", [1, 2])
