@@ -173,3 +173,22 @@ def check(rc: int, what: str) -> None:
         lib = load()
         detail = lib.sa_last_error().decode() or lib.sa_strerror(rc).decode()
         raise SaError(rc, what, detail)
+
+
+# the search entry points with a "_filtered" twin -> the position of their query pointer; the twin takes the same
+# arguments with the filter pointer (sa_filter*) inserted right after it
+QUERY_ARG = {
+    "sa_search": 1, "sa_search_f32": 1, "sa_search_host": 1, "sa_search_host_submit": 2, "sa_search_hits": 1,
+    "sa_sharded_search": 2, "sa_sharded_search_host_submit": 3, "sa_gather_merge": 2, "sa_gather_merge_submit": 3,
+}
+
+
+def search(lib: C.CDLL, name: str, *args, filters=None) -> None:
+    """Call the search entry point ``name``, or with ``filters`` (staged per-query sa_filter words: a numpy array for a
+    host call, a CUDA tensor for a device call) its twin ``name + "_filtered"``.  Raises ``SaError`` naming the symbol
+    called."""
+    if filters is not None:
+        at = QUERY_ARG[name] + 1
+        ptr = filters.data_ptr() if hasattr(filters, "data_ptr") else filters.ctypes.data
+        name, args = name + "_filtered", args[:at] + (ptr,) + args[at:]
+    check(getattr(lib, name)(*args), name)

@@ -47,6 +47,33 @@ def filter_array(filters, nq: int) -> np.ndarray:
     return np.ascontiguousarray(f)
 
 
+def stage_filters(filters, nq: int, device: torch.device | None = None):
+    """A search's ``filters`` where the library reads them: for a host call (``device`` None) the numpy array of
+    ``filter_array``; for a device call an int64 [nq, 4] tensor on ``device``.  Filters already staged there -- an
+    int64 [nq, 4] contiguous CUDA tensor on ``device`` -- are used as is, so a caller can stage them once for many
+    searches.  None (an unfiltered search) stays None."""
+    if not (isinstance(filters, torch.Tensor) and filters.is_cuda):
+        f = None if filters is None else filter_array(filters, nq)
+        return f if f is None or device is None else torch.from_numpy(f.view(np.int64).copy()).to(device)
+    if filters.device != (None if device is None else torch.device(device)):
+        raise ValueError(f"filters on {filters.device} cannot serve a search of queries on {device or 'the host'}")
+    if filters.dtype != torch.int64:
+        raise TypeError(f"device filters must be an int64 tensor of uint64 words, not {filters.dtype}")
+    if tuple(filters.shape) != (nq, 4) or not filters.is_contiguous():
+        raise ValueError(f"device filters must be a contiguous [nq={nq}, 4] tensor, not {list(filters.shape)}")
+    return filters
+
+
+def host_buffers(out, nq: int, k: int, idx_dtype=np.int32):
+    """The (score f32 [nq, k], idx [nq, k]) host buffers of a search: new arrays, or the caller's ``out`` once checked."""
+    if out is None:
+        return np.empty((nq, k), np.float32), np.empty((nq, k), idx_dtype)
+    score, idx = out
+    assert score.shape == (nq, k) and score.dtype == np.float32 and score.flags.c_contiguous
+    assert idx.shape == (nq, k) and idx.dtype == idx_dtype and idx.flags.c_contiguous
+    return score, idx
+
+
 def pinned_array(shape, dtype=np.float32) -> np.ndarray:
     """A page-locked numpy array (sa_host_alloc), freed (sa_host_free) when its last view is garbage-collected."""
     import weakref
@@ -245,99 +272,60 @@ class VectorIndex:
         capi.check(self.lib.sa_corpus_commit(self._h, int(first), int(n), self._stream()), "sa_corpus_commit")
 
     # ------------------------------------------------------------------ search
-    def _filters_dev(self, filters, nq: int, dev) -> torch.Tensor:
-        return torch.from_numpy(filter_array(filters, nq).view(np.int64).copy()).to(dev)
-
     def search(self, q: torch.Tensor, k: int, want_score64: bool = False, filters=None):
         """Device path.  q: [nq, dim] bf16 or fp32 CUDA tensor.  Returns (score f32 [nq,k], idx i32 [nq,k]
         [, score64 f64 [nq,k]]) as CUDA tensors, asynchronous on the current stream.  ``filters`` (uint64 [nq, 4] or
-        [4], see ``filter_array``) restricts each query to the rows whose tag passes its filter."""
+        [4], see ``filter_array``, or an int64 [nq, 4] tensor on q's device, see ``stage_filters``) restricts each query
+        to the rows whose tag passes its filter."""
         assert q.is_cuda and q.dim() == 2 and q.shape[1] == self.dim
+        name = {torch.bfloat16: "sa_search", torch.float32: "sa_search_f32"}.get(q.dtype)
+        if name is None:
+            raise TypeError("queries must be bf16 or fp32")
         q = q.contiguous()
         nq = q.shape[0]
         dev = q.device
         score = torch.empty((nq, k), dtype=torch.float32, device=dev)
         idx = torch.empty((nq, k), dtype=torch.int32, device=dev)
         s64 = torch.empty((nq, k), dtype=torch.float64, device=dev) if want_score64 else None
-        if filters is not None:
-            f = self._filters_dev(filters, nq, dev)
-            if q.dtype == torch.bfloat16:
-                rc = self.lib.sa_search_filtered(self._h, q.data_ptr(), f.data_ptr(), nq, k, score.data_ptr(),
-                                                 idx.data_ptr(), _ptr(s64), self._stream())
-            elif q.dtype == torch.float32:
-                rc = self.lib.sa_search_f32_filtered(self._h, q.data_ptr(), f.data_ptr(), nq, k, score.data_ptr(),
-                                                     idx.data_ptr(), _ptr(s64), self._stream())
-            else:
-                raise TypeError("queries must be bf16 or fp32")
-            capi.check(rc, "sa_search_filtered")
-            return (score, idx, s64) if want_score64 else (score, idx)
-        if q.dtype == torch.bfloat16:
-            rc = self.lib.sa_search(self._h, q.data_ptr(), nq, k, score.data_ptr(), idx.data_ptr(), _ptr(s64),
-                                    self._stream())
-        elif q.dtype == torch.float32:
-            rc = self.lib.sa_search_f32(self._h, q.data_ptr(), nq, k, score.data_ptr(), idx.data_ptr(), _ptr(s64),
-                                        self._stream())
-        else:
-            raise TypeError("queries must be bf16 or fp32")
-        capi.check(rc, "sa_search")
+        capi.search(self.lib, name, self._h, q.data_ptr(), nq, k, score.data_ptr(), idx.data_ptr(), _ptr(s64),
+                    self._stream(), filters=stage_filters(filters, nq, dev))
         return (score, idx, s64) if want_score64 else (score, idx)
 
     def search_host(self, q_f32: np.ndarray, k: int, out=None, filters=None):
         """End-to-end path with HOST buffers (H2D, search, D2H inside the call).  Returns numpy
         (score f32 [nq,k], idx i32 [nq,k]); ``out=(score, idx)`` reuses caller buffers (e.g. ``pinned_array``).
-        ``filters`` as in ``search``."""
+        ``filters`` as in ``search``, as a host array."""
         q = np.ascontiguousarray(q_f32, dtype=np.float32)
         assert q.ndim == 2 and q.shape[1] == self.dim
         nq = q.shape[0]
-        if out is None:
-            score = np.empty((nq, k), dtype=np.float32)
-            idx = np.empty((nq, k), dtype=np.int32)
-        else:
-            score, idx = out
-            assert score.shape == (nq, k) and score.dtype == np.float32 and score.flags.c_contiguous
-            assert idx.shape == (nq, k) and idx.dtype == np.int32 and idx.flags.c_contiguous
+        score, idx = host_buffers(out, nq, k)
         torch.cuda.current_stream(self.device).synchronize()  # the *_host calls run on the engine's stream
-        if filters is not None:
-            f = filter_array(filters, nq)
-            capi.check(self.lib.sa_search_host_filtered(self._h, q.ctypes.data, f.ctypes.data, nq, k, score.ctypes.data,
-                                                        idx.ctypes.data), "sa_search_host_filtered")
-            return score, idx
-        capi.check(self.lib.sa_search_host(self._h, q.ctypes.data, nq, k, score.ctypes.data, idx.ctypes.data),
-                   "sa_search_host")
+        capi.search(self.lib, "sa_search_host", self._h, q.ctypes.data, nq, k, score.ctypes.data, idx.ctypes.data,
+                    filters=stage_filters(filters, nq))
         return score, idx
 
     def search_host_submit(self, q_f32: np.ndarray, k: int, slot: int = 0, filters=None) -> None:
         """First half of ``search_host``: enqueue H2D + search + D2H for ``slot`` (0 or 1) and return at once, so the
         caller can prepare the next batch while the GPU works.  Collect with ``search_host_wait(slot)``.
-        ``filters`` as in ``search`` (staged by the call: the array may be reused at once)."""
+        ``filters`` as in ``search_host`` (staged by the call: the array may be reused at once)."""
         q = np.ascontiguousarray(q_f32, dtype=np.float32)
         assert q.ndim == 2 and q.shape[1] == self.dim
         torch.cuda.current_stream(self.device).synchronize()  # the *_host calls run on the engine's own stream
         self._inflight[slot] = (q, q.shape[0], k)  # keeps a pinned source alive until the wait
-        if filters is not None:
-            f = filter_array(filters, q.shape[0])
-            capi.check(self.lib.sa_search_host_submit_filtered(self._h, slot, q.ctypes.data, f.ctypes.data, q.shape[0],
-                                                               k), "sa_search_host_submit_filtered")
-            return
-        capi.check(self.lib.sa_search_host_submit(self._h, slot, q.ctypes.data, q.shape[0], k),
-                   "sa_search_host_submit")
+        capi.search(self.lib, "sa_search_host_submit", self._h, slot, q.ctypes.data, q.shape[0], k,
+                    filters=stage_filters(filters, q.shape[0]))
 
     def search_host_wait(self, slot: int = 0, out=None):
         _, nq, k = self._inflight.pop(slot)
-        if out is None:
-            score = np.empty((nq, k), dtype=np.float32)
-            idx = np.empty((nq, k), dtype=np.int32)
-        else:
-            score, idx = out
-            assert score.shape == (nq, k) and score.dtype == np.float32 and score.flags.c_contiguous
-            assert idx.shape == (nq, k) and idx.dtype == np.int32 and idx.flags.c_contiguous
+        score, idx = host_buffers(out, nq, k)
         capi.check(self.lib.sa_search_host_wait(self._h, slot, score.ctypes.data, idx.ctypes.data),
                    "sa_search_host_wait")
         return score, idx
 
     def pinned_array(self, shape, dtype=np.float32) -> np.ndarray:
         """A page-locked numpy array (sa_host_alloc): passing such buffers to ``search_host`` lets the engine DMA
-        them directly instead of staging through its own pinned copy.  Freed when the index is closed."""
+        them directly instead of staging through its own pinned copy.  Freed when its last view is garbage-collected,
+        not when the index is closed (see ``close``)."""
         return pinned_array(shape, dtype)
 
     def search_hits(self, q: torch.Tensor, k: int, row_offset: int = 0, filters=None) -> torch.Tensor:
@@ -346,14 +334,8 @@ class VectorIndex:
         assert q.is_cuda and q.dtype == torch.bfloat16 and q.dim() == 2 and q.shape[1] == self.dim
         q = q.contiguous()
         hits = torch.empty((q.shape[0], k, 16), dtype=torch.uint8, device=q.device)
-        if filters is not None:
-            f = self._filters_dev(filters, q.shape[0], q.device)
-            capi.check(self.lib.sa_search_hits_filtered(self._h, q.data_ptr(), f.data_ptr(), q.shape[0], k,
-                                                        int(row_offset), hits.data_ptr(), self._stream()),
-                       "sa_search_hits_filtered")
-            return hits
-        capi.check(self.lib.sa_search_hits(self._h, q.data_ptr(), q.shape[0], k, int(row_offset), hits.data_ptr(),
-                                           self._stream()), "sa_search_hits")
+        capi.search(self.lib, "sa_search_hits", self._h, q.data_ptr(), q.shape[0], k, int(row_offset), hits.data_ptr(),
+                    self._stream(), filters=stage_filters(filters, q.shape[0], q.device))
         return hits
 
     def merge_hits(self, hits_all: torch.Tensor):

@@ -25,6 +25,9 @@ import numpy as np
 import torch
 import torch.distributed as dist
 
+from . import capi
+from .engine import host_buffers, stage_filters
+
 
 def shard_bounds(n_total: int, world: int, rank: int) -> tuple[int, int]:
     """Contiguous, balanced row ranges: rank g owns [g*N//G, (g+1)*N//G)."""
@@ -52,7 +55,6 @@ class ShardedIndex:
 
     # ------------------------------------------------------------------ communicator inside the C ABI
     def _create_comm(self):
-        from . import capi
         lib = self.index.lib
         path = capi.bundled_nccl_path()
         if path:
@@ -89,24 +91,17 @@ class ShardedIndex:
         restricts each query to the rows whose tag passes its filter; each rank's index holds its own rows' tags."""
         nq = q.shape[0]
         if self._comm is not None:
-            from . import capi
             ix = self.index
             q = q.contiguous()
             score = torch.empty((nq, k), dtype=torch.float32, device=q.device)
             rows = torch.empty((nq, k), dtype=torch.int64, device=q.device)
-            if filters is not None:
-                f = ix._filters_dev(filters, nq, q.device)
-                capi.check(ix.lib.sa_sharded_search_filtered(self._comm, ix._h, q.data_ptr(), f.data_ptr(), nq, k,
-                                                             self.row_offset, score.data_ptr(), rows.data_ptr(),
-                                                             ix._stream()), "sa_sharded_search_filtered")
-                return score, rows
-            capi.check(ix.lib.sa_sharded_search(self._comm, ix._h, q.data_ptr(), nq, k, self.row_offset,
-                                                score.data_ptr(), rows.data_ptr(), ix._stream()), "sa_sharded_search")
+            capi.search(ix.lib, "sa_sharded_search", self._comm, ix._h, q.data_ptr(), nq, k, self.row_offset,
+                        score.data_ptr(), rows.data_ptr(), torch.cuda.current_stream(ix.device).cuda_stream,
+                        filters=stage_filters(filters, nq, q.device))
             return score, rows
-        if filters is not None:
-            hits = self.index.search_hits(q, k, self.row_offset, filters=filters)
-        else:
-            hits = self.index.search_hits(q, k, self.row_offset)            # uint8 [nq, k, 16]
+        # an index without filter tags (``search_hits(q, k, row_offset)``) serves the unfiltered searches
+        kw = {} if filters is None else {"filters": filters}
+        hits = self.index.search_hits(q, k, self.row_offset, **kw)            # uint8 [nq, k, 16]
         if self.world == 1:
             return self.index.merge_hits(hits.view(1, nq, k, 16))
         key = (nq, k, str(hits.device))
@@ -123,29 +118,18 @@ class ShardedIndex:
         if self._comm is None:
             self._inflight[slot] = self._search_host_blocking(q, k, filters)
             return
-        from . import capi
-        from .engine import filter_array
         ix = self.index
         self._inflight[slot] = (q, q.shape[0], k)   # keeps a pinned source alive until the wait
-        if filters is not None:
-            f = filter_array(filters, q.shape[0])
-            capi.check(ix.lib.sa_sharded_search_host_submit_filtered(self._comm, ix._h, slot, q.ctypes.data, f.ctypes.data,
-                                                                     q.shape[0], k, self.row_offset),
-                       "sa_sharded_search_host_submit_filtered")
-            return
-        capi.check(ix.lib.sa_sharded_search_host_submit(self._comm, ix._h, slot, q.ctypes.data, q.shape[0], k,
-                                                        self.row_offset), "sa_sharded_search_host_submit")
+        capi.search(ix.lib, "sa_sharded_search_host_submit", self._comm, ix._h, slot, q.ctypes.data, q.shape[0], k,
+                    self.row_offset, filters=stage_filters(filters, q.shape[0]))
 
     def search_host_wait(self, slot: int = 0, out=None):
         got = self._inflight.pop(slot)
         if self._comm is None:
             return got
-        from . import capi
         ix = self.index
         _, nq, k = got
-        if out is None:
-            out = (np.empty((nq, k), np.float32), np.empty((nq, k), np.int64))
-        score, rows = out
+        score, rows = host_buffers(out, nq, k, np.int64)
         capi.check(ix.lib.sa_sharded_search_host_wait(self._comm, ix._h, slot, score.ctypes.data, rows.ctypes.data),
                    "sa_sharded_search_host_wait")
         return score, rows
@@ -153,7 +137,7 @@ class ShardedIndex:
     def _search_host_blocking(self, q: np.ndarray, k: int, filters=None):
         dev = self.index.rows.device if hasattr(self.index, "rows") else torch.device("cpu")
         qd = torch.from_numpy(q).to(dev).to(torch.bfloat16)
-        s, gi = self.search(qd, k) if filters is None else self.search(qd, k, filters=filters)
+        s, gi = self.search(qd, k, filters=filters)
         return s.cpu().numpy(), gi.cpu().numpy()
 
     def search_host(self, q_f32, k: int, out=None, filters=None):
@@ -175,7 +159,6 @@ class MultiGpuIndex:
 
     def __init__(self, dim: int, capacity_per_gpu: int, max_batch: int, max_k: int, n_gpus: int | None = None,
                  similarity: str = "cosine"):
-        from . import capi
         from .engine import VectorIndex
         n = torch.cuda.device_count() if n_gpus is None else int(n_gpus)
         if n < 1 or n > torch.cuda.device_count():
@@ -267,32 +250,20 @@ class MultiGpuIndex:
 
     def search_host_submit(self, q_f32: np.ndarray, k: int, slot: int = 0, filters=None) -> None:
         """``filters`` (uint64 [nq, 4] or [4]) applies to every shard, each filtering its rows by its own tags."""
-        from . import capi
-        from .engine import filter_array
         q = np.ascontiguousarray(q_f32, dtype=np.float32)
         self._inflight[slot] = (q, q.shape[0], k)
-        if filters is not None:
-            f = filter_array(filters, q.shape[0])
-            capi.check(self.lib.sa_gather_merge_submit_filtered(self._comm, self._engines, slot, q.ctypes.data,
-                                                                f.ctypes.data, q.shape[0], k, self._offsets),
-                       "sa_gather_merge_submit_filtered")
-            return
-        capi.check(self.lib.sa_gather_merge_submit(self._comm, self._engines, slot, q.ctypes.data, q.shape[0], k,
-                                                   self._offsets), "sa_gather_merge_submit")
+        capi.search(self.lib, "sa_gather_merge_submit", self._comm, self._engines, slot, q.ctypes.data, q.shape[0], k,
+                    self._offsets, filters=stage_filters(filters, q.shape[0]))
 
     def search_host_wait(self, slot: int = 0, out=None):
         """(score f32 [nq, k], dense row i64 [nq, k]); ties between shards resolve by the library's global row order
         (shard, then local row), not by dense id."""
-        from . import capi
         _, nq, k = self._inflight.pop(slot)
-        score = np.empty((nq, k), np.float32) if out is None else out[0]
+        score, dense = host_buffers(out, nq, k, np.int64)
         rows = np.empty((nq, k), np.int64)
         capi.check(self.lib.sa_gather_merge_wait(self._comm, self._engines, slot, score.ctypes.data, rows.ctypes.data),
                    "sa_gather_merge_wait")
-        dense = self._to_dense(rows)
-        if out is not None:
-            out[1][:] = dense
-            return out
+        dense[:] = self._to_dense(rows)
         return score, dense
 
     def search_host(self, q_f32: np.ndarray, k: int, out=None, filters=None):

@@ -31,59 +31,73 @@ for p in (ROOT, os.path.join(ROOT, "tests")):
         sys.path.insert(0, p)
 
 import bench  # noqa: E402
+from harness.filter_oracle import eligibility  # noqa: E402
 from harness.similarity_oracle import SIMILARITIES, RunningTopk, internal_scores  # noqa: E402
 
 PIECE = 65_536
+PROG = os.path.splitext(os.path.basename(sys.argv[0]))[0]
 
 
 def _w_prefilter(task):
-    """fp32 prefilter of one piece of the shared corpus: per similarity, the piece's `keep` best rows per query."""
+    """fp32 prefilter of one piece of the shared corpus: per (similarity, case), the piece's `keep` best eligible rows
+    per query, with their fp32 values (-inf: not eligible)."""
     from oracle import bruteforce as bf
-    q_bits, first, off, rows, dim, keep = task
+    q_bits, first, off, rows, dim, keep, sims, tags, filters = task
     q = bf.bf16_bits_to_f32(q_bits)
     c = bf.bf16_bits_to_f32(bench._shared_view(off, rows, dim))
     dots = (q @ c.T).astype(np.float64)
     qq = (q.astype(np.float64) ** 2).sum(axis=1)
     cc = np.einsum("ij,ij->i", c, c, dtype=np.float64)
     out = {}
-    for sim in SIMILARITIES:
-        s = internal_scores(sim, dots, qq, cc)
-        kk = min(keep, s.shape[1])
-        part = np.argpartition(s, s.shape[1] - kk, axis=1)[:, s.shape[1] - kk:]
-        out[sim] = part.astype(np.int64) + first
+    for sim in sims:
+        s0 = internal_scores(sim, dots, qq, cc)
+        for case, f in filters.items():
+            s = s0
+            if f is not None:
+                s = s0.copy()
+                s[~eligibility(tags, f)] = -np.inf
+            kk = min(keep, s.shape[1])
+            part = np.argpartition(s, s.shape[1] - kk, axis=1)[:, s.shape[1] - kk:]
+            out[(sim, case)] = (part.astype(np.int64) + first, np.take_along_axis(s, part, axis=1))
     return out
 
 
-def exact_topk(host, q_bits, n_rows, dim, k, margin=64):
-    """{similarity: row int64 [nq, k]} over all n_rows rows of the host copy: an fp32 prefilter keeps k + margin rows
-    per query and piece (spread over the pool), then those candidates are re-scored in float64 (the definition) and
-    selected by (value desc, row asc).  Equal to the definition unless more than `margin` rows of one piece sit within
-    fp32 rounding (~1e-6 relative) of a query's k-th value."""
+def exact_topk(host, q_bits, n_rows, dim, k, sims=SIMILARITIES, filtered=None, margin=64):
+    """Row int64 [nq, k] (-1 = empty slot) of the float64 definition over all n_rows rows of the host copy, per
+    similarity: {similarity: rows}; with ``filtered`` = (tags uint64 [n_rows], {case: filters uint64 [nq, 4] or None}),
+    per similarity and case over each query's eligible rows: {(similarity, case): rows}.  An fp32 prefilter keeps
+    k + margin rows per query and piece (spread over the pool), then those candidates are re-scored in float64 (the
+    definition) and selected by (value desc, row asc).  Equal to the definition unless more than `margin` rows of one
+    piece sit within fp32 rounding (~1e-6 relative) of a query's k-th value."""
     from oracle import bruteforce as bf
-    tasks = [(q_bits, lo, lo * dim * 2, min(PIECE, n_rows - lo), dim, k + margin) for lo in range(0, n_rows, PIECE)]
-    cand = {sim: [] for sim in SIMILARITIES}
+    tags, filters = filtered if filtered is not None else (None, {None: None})
+    tasks = [(q_bits, lo, lo * dim * 2, min(PIECE, n_rows - lo), dim, k + margin, sims,
+              None if tags is None else tags[lo:lo + PIECE], filters) for lo in range(0, n_rows, PIECE)]
+    cand = {}
     for part in host.pool.imap_unordered(_w_prefilter, tasks, chunksize=1):
-        for sim, rows in part.items():
-            cand[sim].append(rows)
+        for key, (rows, vals) in part.items():
+            cand.setdefault(key, []).append(np.where(np.isfinite(vals), rows, -1))
     shard = host.view(n_rows, dim)
     q = bf.bf16_bits_to_f32(q_bits).astype(np.float64)
     out = {}
-    for sim in SIMILARITIES:
-        rows_all = np.concatenate(cand[sim], axis=1)
+    for (sim, case), parts in cand.items():
+        rows_all = np.concatenate(parts, axis=1)
         res = np.full((len(q), k), -1, dtype=np.int64)
         for r in range(len(q)):
-            rows = np.unique(rows_all[r])
+            rows = np.unique(rows_all[r][rows_all[r] >= 0])
+            if len(rows) == 0:
+                continue
             c = bf.bf16_bits_to_f32(shard[rows]).astype(np.float64)
             acc = RunningTopk(1, k)
             s = internal_scores(sim, (c @ q[r])[None, :], np.array([q[r] @ q[r]]), (c * c).sum(axis=1))
             acc.add(s, 0)
             res[r] = np.where(acc.i[0] >= 0, rows[np.maximum(acc.i[0], 0)], -1)
-        out[sim] = res
+        out[sim if filtered is None else (sim, case)] = res
     return out
 
 
 def log(msg):
-    print(f"[similarity_bench {time.strftime('%H:%M:%S')}] {msg}", file=sys.stderr, flush=True)
+    print(f"[{PROG} {time.strftime('%H:%M:%S')}] {msg}", file=sys.stderr, flush=True)
 
 
 def gpu_identity():
@@ -98,65 +112,94 @@ def gpu_identity():
     return name, power
 
 
-def run_shape(host, n, dim, B, k, a, name, power):
+def indexes(host, n, dim, B, max_k, sims, a):
+    """(similarity, index, q_bits, qd) per similarity over one corpus: bench.py's recipe uploaded into the first index
+    (HostData + upload, mirrored to the host copy) and copied device to device into each next one, which closes the
+    one before; bench.py's queries (odd ones planted near rows of the first chunk), as bf16 bits and on the device."""
     import torch
     from oracle import bruteforce as bf
     from qsa_b200.engine import VectorIndex
-    sample = min(a.sample, B)
-    oracle_s = None
-    prev = None
-    for sim in SIMILARITIES:
-        ix = VectorIndex(dim=dim, capacity=n, max_batch=B, max_k=k, similarity=sim)
+    prev = q_bits = qd = None
+    for sim in sims:
+        ix = VectorIndex(dim=dim, capacity=n, max_batch=B, max_k=max_k, similarity=sim)
         log(f"{n}x{dim} b{B}: {sim}")
         if prev is None:
             bench.upload(host, ix, torch, a.seed, dim, 0, n, n, a.data)
-            # bench.py's query recipe: odd queries are planted near rows of the corpus' first chunk (now in the host copy)
             q_bits = bf.synth_queries(a.seed + 1, B, dim, host.view(min(n, bench.CHUNK), dim))
             qd = torch.from_numpy(q_bits.view(np.int16)).view(torch.bfloat16).cuda()
-            log("uploaded; exact answers for the query sample")
-            t0 = time.perf_counter()
-            ref = exact_topk(host, q_bits[:sample], n, dim, k)
-            oracle_s = time.perf_counter() - t0
-            log(f"oracle {oracle_s:.0f} s")
         else:
             ix.rows[:n].copy_(prev.rows[:n])                   # the same bits, device to device
             prev.close()
-            del prev
             ix.commit(0, n)
         torch.cuda.synchronize()
-        for _ in range(a.warmup):
-            ix.search(qd, k)
-        torch.cuda.synchronize()
-        ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        ev0.record()
-        for _ in range(a.steps):
-            ix.search(qd, k)
-        ev1.record()
-        torch.cuda.synchronize()
-        ms = ev0.elapsed_time(ev1) / a.steps
-        scan_ms, total_ms, used = ix.timing_mean(min(a.steps, 16))
-        ix.set_option("count_fix", 1)
-        s, i = ix.search(qd, k)                                # untimed: exactness and fallback work
-        torch.cuda.synchronize()
-        fix = ix.info("last_fix_entries")
-        ix.set_option("count_fix", 0)
-        got = i.cpu().numpy()[:sample].astype(np.int64)
-        want = ref[sim]
-        recall = float(np.mean([len(np.intersect1d(got[r], want[r])) / k for r in range(sample)]))
-        print(json.dumps({
-            "workload": f"{n}x{dim}_b{B}_k{k}", "similarity": sim, "qps": round(B / (ms * 1e-3), 1),
-            "ms_per_batch": round(ms, 3), "scan_ms": round(scan_ms, 3), "total_ms_engine": round(total_ms, 3),
-            "recall": recall, "strict_order": float((got == want).all(axis=1).mean()), "recall_queries": sample,
-            "last_fix_entries": int(fix), "steps": a.steps, "warmup": a.warmup, "data": a.data,
-            "gpu": name, "power_limit_w": power, "oracle_s": round(oracle_s, 1)}), flush=True)
+        yield sim, ix, q_bits, qd
         prev = ix
     prev.close()
 
 
-def main(argv=None) -> int:
-    ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
-    ap.add_argument("--shapes", default="1000000x1536x256,10000000x1536x1024", help="ROWSxDIMxBATCH,...")
-    ap.add_argument("--k", type=int, default=10)
+def timed_case(ix, qd, k, a, filters=None):
+    """One case with bench.py's step discipline: the filters staged on the device once, W untimed searches, then K
+    searches between CUDA events; the engine's mean scan and total ms over them; one more untimed search with
+    count_fix = 1 for exactness and fallback work.  Returns (timing fields, last_fix_entries, its rows int64 [nq, k])."""
+    import torch
+    from qsa_b200.engine import stage_filters
+    f = stage_filters(filters, qd.shape[0], qd.device)
+    for _ in range(a.warmup):
+        ix.search(qd, k, filters=f)
+    torch.cuda.synchronize()
+    ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    ev0.record()
+    for _ in range(a.steps):
+        ix.search(qd, k, filters=f)
+    ev1.record()
+    torch.cuda.synchronize()
+    ms = ev0.elapsed_time(ev1) / a.steps
+    scan_ms, total_ms, _ = ix.timing_mean(min(a.steps, 16))
+    ix.set_option("count_fix", 1)
+    _, i = ix.search(qd, k, filters=f)
+    torch.cuda.synchronize()
+    fix = ix.info("last_fix_entries")
+    ix.set_option("count_fix", 0)
+    timing = {"qps": round(qd.shape[0] / (ms * 1e-3), 1), "ms_per_batch": round(ms, 3), "scan_ms": round(scan_ms, 3),
+              "total_ms_engine": round(total_ms, 3)}
+    return timing, int(fix), i.cpu().numpy().astype(np.int64)
+
+
+def report(head, timing, fix, got, want, a, gpu, **tail):
+    """Print a case's JSON line: ``head``, ``timing``, recall and strict order of the first len(want) result rows
+    against ``want`` (-1 = empty slot), the run's settings and the GPU's (name, power limit), then ``tail``."""
+    got = got[:len(want)]
+    recall = float(np.mean([
+        len(np.intersect1d(got[r][got[r] >= 0], want[r][want[r] >= 0])) / max(1, int((want[r] >= 0).sum()))
+        for r in range(len(want))]))
+    print(json.dumps({
+        **head, **timing, "recall": recall, "strict_order": float((got == want).all(axis=1).mean()),
+        "recall_queries": len(want), "last_fix_entries": fix, "steps": a.steps, "warmup": a.warmup, "data": a.data,
+        "gpu": gpu[0], "power_limit_w": gpu[1], **tail}), flush=True)
+
+
+def run_shape(host, n, dim, B, a, gpu):
+    sample = min(a.sample, B)
+    ref = None
+    for sim, ix, q_bits, qd in indexes(host, n, dim, B, a.k, SIMILARITIES, a):
+        if ref is None:
+            log("uploaded; exact answers for the query sample")
+            t0 = time.perf_counter()
+            ref = exact_topk(host, q_bits[:sample], n, dim, a.k)
+            oracle_s = time.perf_counter() - t0
+            log(f"oracle {oracle_s:.0f} s")
+        timing, fix, got = timed_case(ix, qd, a.k, a)
+        report({"workload": f"{n}x{dim}_b{B}_k{a.k}", "similarity": sim}, timing, fix, got, ref[sim], a, gpu,
+               oracle_s=round(oracle_s, 1))
+
+
+def main(argv=None, doc=__doc__, run_shape=run_shape, shapes="1000000x1536x256,10000000x1536x1024",
+         add_args=lambda ap: ap.add_argument("--k", type=int, default=10)) -> int:
+    """The bench harnesses' command line: ``add_args`` adds a harness's own options, then ``run_shape(host, n, dim, B,
+    args, (gpu name, power limit))`` runs for each ROWSxDIMxBATCH of --shapes over one shared host copy."""
+    ap = argparse.ArgumentParser(description=doc, formatter_class=argparse.RawDescriptionHelpFormatter)
+    ap.add_argument("--shapes", default=shapes, help="ROWSxDIMxBATCH,...")
+    add_args(ap)
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--sample", type=int, default=16, help="queries of the batch checked against the exact definition")
@@ -170,10 +213,10 @@ def main(argv=None) -> int:
     try:
         import torch
         if not torch.cuda.is_available():
-            raise SystemExit("similarity_bench needs a CUDA device (H100); there is no CPU fallback")
-        name, power = gpu_identity()
+            raise SystemExit(f"{PROG} needs a CUDA device (H100); there is no CPU fallback")
+        gpu = gpu_identity()
         for n, d, B in shapes:
-            run_shape(host, n, d, B, a.k, a, name, power)
+            run_shape(host, n, d, B, a, gpu)
     finally:
         host.close()
     return 0

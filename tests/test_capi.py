@@ -110,3 +110,20 @@ def test_launch_planner_headline_shapes(lib):
     p = plan(lib, 132, 4096, 2, 4883)                                       # config 4 per GPU: 6 launches
     assert [x[2:] for x in p] == [(3, 22)] * 4 + [(2, 33)] * 2
     assert len(plan(lib, 132, 1100, 2, 118, cap=2)) == 3                    # forced small launches
+
+
+def test_filtered_twins_take_the_filter_right_after_the_query(lib):
+    """Every X_filtered is X with one sa_filter* inserted right after the query pointer -- the rule capi.search relies
+    on -- in the binding's signatures and in the header's parameter names."""
+    twins = sorted(n[:-len("_filtered")] for n in capi.EXPORTS if n.endswith("_filtered"))
+    assert twins == sorted(capi.QUERY_ARG)
+    src = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "sa_api.h")).read(), flags=re.S)
+    params = {m[0]: [p.split()[-1].lstrip("*") for p in m[1].split(",")]
+              for m in re.findall(r"\b(sa_[a-z0-9_]+)\s*\(([^)]*)\)", src)}
+    for name in twins:
+        at = capi.QUERY_ARG[name] + 1
+        base, twin = list(getattr(lib, name).argtypes), list(getattr(lib, name + "_filtered").argtypes)
+        assert twin == base[:at] + [C.c_void_p] + base[at:], name
+        assert params[name][at - 1].startswith("q_"), (name, params[name])
+        f = params[name + "_filtered"][at]
+        assert f.startswith("filters_") and params[name + "_filtered"] == params[name][:at] + [f] + params[name][at:], name

@@ -269,3 +269,32 @@ def test_oracle_reproduces_the_independent_fixture(path):
         assert (i == z[f"{key}_idx"]).all(), sim
         fin = np.isfinite(z[f"{key}_score"])
         assert (np.abs(s - z[f"{key}_score"])[fin] < 1e-9).all()
+
+
+def test_bench_harness_exact_topk_equals_the_definitions():
+    """The bench harnesses' exact_topk (fp32 prefilter per piece + float64 rescoring) over bench.HostData at three
+    pieces equals similarity_oracle.topk_f64 per similarity and, with filters, filter_oracle.topk_f64 -- including a
+    filter no row passes."""
+    import bench
+    from harness import similarity_oracle
+    from harness.similarity_bench import PIECE, exact_topk
+    from oracle import bruteforce as bf
+    n, dim, nq, k, seed = 2 * PIECE + 1000, 64, 6, 12, 5
+    tags = np.random.default_rng(seed).integers(0, 4, n).astype(np.uint64)
+    filters = {"bit0": np.tile(np.array([1, 0, 0, 0], np.uint64), (nq, 1)),
+               "none": np.tile(np.array([8, 0, 0, 0], np.uint64), (nq, 1))}
+    host = bench.HostData(n * dim * 2, 2)
+    try:
+        host.generate(seed, dim, 0, n, n)
+        c_bits = host.view(n, dim)
+        q_bits = bf.synth_queries(seed + 1, nq, dim, c_bits[:1000])
+        plain = exact_topk(host, q_bits, n, dim, k)
+        filtered = exact_topk(host, q_bits, n, dim, k, similarity_oracle.SIMILARITIES, (tags, filters))
+        for sim in similarity_oracle.SIMILARITIES:
+            assert (plain[sim] == similarity_oracle.topk_f64(q_bits, c_bits, k, sim)[1]).all(), sim
+            for case, f in filters.items():
+                want = topk_f64(q_bits, c_bits, k, sim, eligibility(tags, f))[1]
+                assert (filtered[(sim, case)] == want).all(), (sim, case)
+        assert (filtered[("cosine", "none")] == -1).all()
+    finally:
+        host.close()

@@ -253,6 +253,28 @@ def test_host_slots_hits_and_snapshot(bf, sim, tmp_path):
     compare(s1, i1, *r1)
     hs, hi = ix.search_host(qf[:70], k, filters=fa)
     compare(hs, hi, *r0)
+    # fp32 device queries, unfiltered and filtered; filters staged on the device give the numpy form's bits
+    fd = torch.from_numpy(np.tile(fb, (nq, 1)).view(np.int64)).cuda()
+    rb = topk_f64(q, c, k, sim, eligibility(tags, np.tile(fb, (nq, 1))))
+    for filters, want in ((None, topk_f64(q, c, k, sim, np.ones((nq, n), bool))), (fb, rb), (fd, rb)):
+        s, i = ix.search(torch.from_numpy(qf).cuda(), k, filters=filters)
+        torch.cuda.synchronize()
+        compare(s.cpu().numpy(), i.cpu().numpy(), *want)
+    (sn, i_n), (sd, i_d) = ix.search(dev(q), k, filters=fb), ix.search(dev(q), k, filters=fd)
+    assert torch.equal(sn, sd) and torch.equal(i_n, i_d)
+    for bad, err in ((fd[:10], ValueError), (fd.int(), TypeError), (fd.t().contiguous().t(), ValueError)):
+        with pytest.raises(err):
+            ix.search(dev(q), k, filters=bad)
+    with pytest.raises(ValueError, match="host"):
+        ix.search_host(qf, k, filters=fd)                       # device filters cannot serve a host-buffer search
+    # a one-GPU ShardedIndex (torch transport): search_hits + merge_hits
+    from qsa_b200.sharded import ShardedIndex
+    sh = ShardedIndex(ix, row_offset=0)
+    assert sh.transport == "torch"
+    s, i = sh.search(dev(q), k, filters=fb)
+    torch.cuda.synchronize()
+    compare(s.cpu().numpy(), i.cpu().numpy(), *rb)
+    compare(*sh.search_host(qf, k, filters=fb), *rb)
     # two shards on one GPU through the packed exchange
     cut = 3100
     a, b = index(sim, dim, cut, max_batch=256, max_k=k), index(sim, dim, n - cut, max_batch=256, max_k=k)

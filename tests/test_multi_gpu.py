@@ -50,6 +50,17 @@ def test_single_process_gather_merge_equals_oracle(n):
     for slot, j in ((0, 1), (1, 2)):
         s, i = mi.search_host_wait(slot)
         assert (i == refs[j][1]).all() and np.abs(s.astype(np.float64) - refs[j][0]).max() < 1e-6
+    # filtered, host call and submit / wait: each shard filters its own rows by their tags
+    from harness.filter_oracle import eligibility, topk_f64
+    tags = g.integers(0, 4, len(mi)).astype(np.uint64)
+    mi.set_tags(np.arange(len(mi)), tags)
+    f = np.zeros((37, 4), np.uint64)
+    f[:, 0], f[::2, 1] = 1, 2
+    want = topk_f64(batches[1], c, k, "cosine", eligibility(tags, f))[1]
+    assert (mi.search_host(f32[1], k, filters=f)[1] == want).all()
+    mi.search_host_submit(f32[1], k, 1, filters=f)
+    out = (np.empty((37, k), np.float32), np.empty((37, k), np.int64))
+    assert mi.search_host_wait(1, out=out)[1] is out[1] and (out[1] == want).all()
     mi.delete_rows([int(refs[0][1][0, 0])])                       # tombstone the best hit of query 0: the runner-up moves up
     s, i = mi.search_host(f32[0][:1], k)
     assert i[0, 0] == refs[0][1][0, 1]
