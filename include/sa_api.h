@@ -47,6 +47,19 @@ typedef enum sa_status {
 #define SA_SIM_DOT 1
 #define SA_SIM_EUCLIDEAN 2
 
+/* Element type of an index, fixed at creation: the type of its rows and of the queries of its device search forms.
+ *   SA_ELEM_BF16  rows and queries are bf16 (sa_engine_create, sa_engine_create_sim)
+ *   SA_ELEM_INT8  rows and queries are int8 (Atlas's int8 vectors, pre-quantized int8 embeddings).  The definition above
+ *                 is evaluated on the integers themselves; every sum is exact, so cosine is <q,c> / sqrt(|q|^2 |c|^2),
+ *                 dotProduct the integer <q,c>, and the distance one correctly rounded sqrt of an exact integer.  There
+ *                 is no scale factor: scores are in the integers' own units.  fp32 input to an int8 index (the *_f32
+ *                 and *_host forms, sa_gather_merge*) is converted by one rule: round to nearest even, saturate to
+ *                 [-128, 127], NaN -> 0 (sa_debug_int8_round), so integer-valued floats in range pass unchanged.
+ * Pointers documented below as "*_bf16_dev" (the rows of sa_corpus_bind, the queries of sa_search, sa_search_filtered,
+ * sa_search_hits*, sa_sharded_search* and sa_debug_tile_dots) point to elements of the engine's type. */
+#define SA_ELEM_BF16 0
+#define SA_ELEM_INT8 1
+
 /* Largest k of a search.  Candidate lists hold 16 (k <= 16) or 32 entries per tile lane; a "deep" search (28 < k <= 64)
  * keeps the 32-entry lists and runs a scan variant whose shared bounds hold for its k (DESIGN.md section 4.1). */
 #define SA_MAX_K 64
@@ -64,15 +77,20 @@ const char* sa_last_error(void); /* thread-local detail of the last failure on t
  *   (assets/pre-setup/MongoDB-Setup.md:72-83, scripts/common/validate.py:56-61,167-180).
  * dim must be a multiple of 64 (1536 and 768 are); capacity_rows < 2^31; max_k <= SA_MAX_K.  sa_engine_create makes a
  * cosine index; sa_engine_create_sim takes the similarity (SA_SIM_*) and rejects any other value with SA_ERR_ARG before
- * it touches a device. */
+ * it touches a device.  sa_engine_create_elem also takes the element type (SA_ELEM_*; sa_engine_create_sim is it with
+ * SA_ELEM_BF16); an int8 index needs dim to be a multiple of 128 and at most 65536 (so |<q,c>| <= dim 2^14 fits in
+ * int32).  An unknown elem or such a dim is rejected with SA_ERR_ARG before it touches a device. */
 int sa_engine_create(sa_engine** out, int device, int dim, int64_t capacity_rows, int max_batch, int max_k);
 int sa_engine_create_sim(sa_engine** out, int device, int dim, int64_t capacity_rows, int max_batch, int max_k,
                          int similarity);
+int sa_engine_create_elem(sa_engine** out, int device, int dim, int64_t capacity_rows, int max_batch, int max_k,
+                          int similarity, int elem);
 void sa_engine_destroy(sa_engine* e);
 
-/* Attach caller-owned device storage: rows_bf16 is [capacity_rows x dim] row-major bf16 (16-byte aligned),
- * row_term is [capacity_rows] fp32 (16-byte aligned), one term per row that the scan combines with <q,c>:
- *   cosine      1/|c| over the bf16 values, 0 for an all-zero row or a tombstone
+/* Attach caller-owned device storage: rows_bf16 is [capacity_rows x dim] row-major of the engine's element type (bf16
+ * or int8; 16-byte aligned), row_term is [capacity_rows] fp32 (16-byte aligned), one term per row that the scan
+ * combines with <q,c>:
+ *   cosine      1/|c| over the stored values (int8: rounded once from fp64), 0 for an all-zero row or a tombstone
  *   dotProduct  1 for a live row, 0 for a tombstone
  *   euclidean   |c|^2/2 (summed in fp64, rounded once to fp32) for a live row, negative (e.g. -1) for a tombstone
  * The ingest entry points below write it; a caller that tombstones a row writes the row's term itself (and may zero the
@@ -101,10 +119,11 @@ typedef struct sa_filter {
 
 /* --- ingest (the "documents -> documents_embed -> MongoDB sink" half of Lab2, LAB2-Walkthrough.md:41-51,
  *     fed by scripts/publish_docs.py:225-351; embeddings arrive as ARRAY<FLOAT>, main.tf:141,215) ------- */
-/* Rows [first_row, first_row+n_new) were written in place as bf16 by the caller: compute their row terms and
- * publish them (first_row must equal the current row count). */
+/* Rows [first_row, first_row+n_new) were written in place (bf16 or int8, the engine's element type) by the caller:
+ * compute their row terms and publish them (first_row must equal the current row count). */
 int sa_corpus_commit(sa_engine* e, int64_t first_row, int64_t n_new, uintptr_t stream);
-/* Convert n_new fp32 rows (device) to bf16 (round-to-nearest-even), append, compute row terms, publish. */
+/* Convert n_new fp32 rows (device) to the element type (bf16: round-to-nearest-even; int8: see SA_ELEM_INT8), append,
+ * compute row terms, publish. */
 int sa_corpus_append_f32(sa_engine* e, const float* rows_f32_dev, int64_t n_new, uintptr_t stream);
 /* Same from host memory (staged through pinned memory in chunks); blocking. */
 int sa_corpus_append_host_f32(sa_engine* e, const float* rows_f32_host, int64_t n_new);
@@ -123,7 +142,8 @@ int64_t sa_corpus_rows(const sa_engine* e);
  * out_score64 (optional, may be NULL) receives the unrounded scores for a cross-shard merge. */
 int sa_search(sa_engine* e, const void* q_bf16_dev, int nq, int k, float* out_score_dev, int32_t* out_idx_dev,
               double* out_score64_dev, uintptr_t stream);
-/* Queries as fp32 (the ML_PREDICT output type, terraform/core/main.tf:500,534): rounded to bf16 first. */
+/* Queries as fp32 (the ML_PREDICT output type, terraform/core/main.tf:500,534): converted to the element type first
+ * (bf16: round-to-nearest-even; int8: see SA_ELEM_INT8).  The host forms below convert the same way. */
 int sa_search_f32(sa_engine* e, const float* q_f32_dev, int nq, int k, float* out_score_dev, int32_t* out_idx_dev,
                   double* out_score64_dev, uintptr_t stream);
 /* End-to-end call with HOST buffers: H2D of the queries, search, D2H of the results; blocking. */
@@ -220,7 +240,8 @@ int sa_gather_merge_submit_filtered(sa_comm* c, sa_engine* const* engines, int s
 /* --- observability ------------------------------------------------------------------------------------
  * CUDA-event times of the most recent search on this engine (synchronises on its last event):
  * scan_ms = sum over its scan-kernel launches, total_ms = first scan start to last merge end,
- * bytes / flops = ALGORITHMIC work of that search (DESIGN.md section 5), launches = scan launches,
+ * bytes / flops = ALGORITHMIC work of that search (DESIGN.md section 5; rows and queries at 2 bytes per bf16 element,
+ * 1 per int8 element; for an int8 engine "flops" are int8 operations, same formula), launches = scan launches,
  * kernels = all kernels the search launched. */
 int sa_last_timing(sa_engine* e, float* scan_ms, float* total_ms, double* bytes, double* flops, int* launches,
                    int* kernels);
@@ -243,7 +264,8 @@ int sa_timing_mean(sa_engine* e, int n, float* scan_ms_mean, float* total_ms_mea
  * "count_fix" = 0 | 1 (record how many (query, lane) pairs the last search sent to the fallback; costs a host sync). */
 int sa_set_option(sa_engine* e, const char* name, int64_t value);
 /* "num_sms", "dim", "capacity", "n_rows", "max_batch", "max_k", "last_grid", "last_fix_entries" (with "count_fix"),
- * "eps_rel_e12" (the certificate's relative error bound, times 1e12), "similarity" (SA_SIM_*), "cmax_bits" (fp32 bits of
+ * "eps_rel_e12" (the certificate's relative error bound, times 1e12; int8: a constant, DESIGN.md section 4.2),
+ * "similarity" (SA_SIM_*), "elem" (SA_ELEM_*), "cmax_bits" (fp32 bits of
  * the device-side upper bound on the committed rows' norms; dotProduct and euclidean only, 0 for cosine; synchronous),
  * "has_tags" (1 when a row tag array is bound, sa_corpus_bind_tags). */
 int sa_get_info(const sa_engine* e, const char* name, int64_t* value);
@@ -252,7 +274,8 @@ int sa_get_info(const sa_engine* e, const char* name, int64_t* value);
  * epilogue wait for the MMA, epilogue busy, epilogue 32-column chunks on the insertion path, CTA lifetime, tiles}, SM cycles. */
 int sa_scan_profile(sa_engine* e, int64_t* out_host, int max_ctas, int* n_ctas);
 
-/* Test hook: raw fp32 Q.C^T accumulators of one 256-row corpus tile for the first nq queries,
+/* Test hook: raw fp32 Q.C^T accumulators (int8: the exact int32 accumulators rounded to fp32) of one 256-row corpus tile
+ * for the first nq queries (of the engine's element type),
  * out_dots_dev is [ceil(nq/(128*cg))*128*cg x 256].  Runs the scan kernel's debug instantiation. */
 int sa_debug_tile_dots(sa_engine* e, const void* q_bf16_dev, int nq, int tile, int cta_group, float* out_dots_dev,
                        uintptr_t stream);
@@ -269,6 +292,8 @@ int sa_debug_plan(int num_sms, int nq, int cta_group, int num_tiles, int max_lau
  * receives the "dropped" bound: the largest score the list saw and does not hold. */
 int sa_debug_float_keys(const float* x, int n, uint32_t* key, float* back, float* below);
 int sa_debug_bf16_round(const float* x, int n, uint16_t* bits, float* back);
+/* The fp32 -> int8 conversion of an int8 index (SA_ELEM_INT8): round to nearest even, saturate, NaN -> 0. */
+int sa_debug_int8_round(const float* x, int n, int8_t* out);
 int sa_debug_merge_keys(const float* score, const int32_t* row, int n, uint64_t* key, int32_t* row_back);
 int sa_debug_list_insert(const float* score, const int32_t* row, int n, int list_len, const float* floor_after,
                          float* out_score, int32_t* out_row, float* out_drop);

@@ -27,10 +27,23 @@ SA_SIM_EUCLIDEAN = 2
 SIMILARITIES = {"cosine": SA_SIM_COSINE, "dotProduct": SA_SIM_DOT, "euclidean": SA_SIM_EUCLIDEAN}
 
 
+SA_ELEM_BF16 = 0
+SA_ELEM_INT8 = 1
+# an index's element type (the dtype of its rows and device queries) -> the engine's constants
+ELEMS = {"bfloat16": SA_ELEM_BF16, "int8": SA_ELEM_INT8}
+
+
 def similarity_code(name: str) -> int:
     if name not in SIMILARITIES:
         raise ValueError(f"similarity must be one of {sorted(SIMILARITIES)}, not {name!r}")
     return SIMILARITIES[name]
+
+
+def elem_code(name: str) -> int:
+    if name not in ELEMS:
+        raise ValueError(f"dtype must be one of {sorted(ELEMS)}, not {name!r}")
+    return ELEMS[name]
+
 
 # every symbol include/sa_api.h declares (tests check the .so exports each of them)
 EXPORTS = (
@@ -51,6 +64,8 @@ EXPORTS = (
     "sa_search_host_submit_filtered", "sa_search_hits_filtered", "sa_sharded_search_filtered",
     "sa_sharded_search_host_submit_filtered", "sa_gather_merge_filtered", "sa_gather_merge_submit_filtered",
     "sa_debug_filter_pass",
+    # int8 indexes
+    "sa_engine_create_elem", "sa_debug_int8_round",
     # include/sa_wire.h
     "sa_wire_split_log", "sa_wire_decode_queries_embed", "sa_wire_decode_documents_embed", "sa_wire_encode_search_results", "sa_wire_encode_queries_embed",
 )
@@ -145,6 +160,8 @@ def load() -> C.CDLL:
         "sa_gather_merge_filtered": (i32, [vp, C.POINTER(vp), vp, vp, i32, i32, C.POINTER(i64), vp, vp]),
         "sa_gather_merge_submit_filtered": (i32, [vp, C.POINTER(vp), i32, vp, vp, i32, i32, C.POINTER(i64)]),
         "sa_debug_filter_pass": (i32, [vp, i32, vp, vp]),
+        "sa_engine_create_elem": (i32, [C.POINTER(vp), i32, i32, i64, i32, i32, i32, i32]),
+        "sa_debug_int8_round": (i32, [vp, i32, vp]),
         "sa_host_alloc": (i32, [C.POINTER(vp), u64]),
         "sa_host_free": (i32, [vp]),
     }

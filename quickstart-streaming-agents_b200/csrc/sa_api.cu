@@ -72,15 +72,17 @@ EncodeTiledFn get_encode_fn() {
   return fn;
 }
 
-// 2-D bf16 tensor [rows x dim], box = 64 columns (128 B, SWIZZLE_128B) x box_rows rows.
-int encode_rows_map(CUtensorMap* m, const void* base, uint64_t rows, int dim, int box_rows) {
+// 2-D tensor [rows x dim] of the engine's element type, box = one 128-B K slice (SWIZZLE_128B: 64 bf16 or 128 int8
+// columns) x box_rows rows.
+int encode_rows_map(CUtensorMap* m, const void* base, uint64_t rows, int dim, int box_rows, int elem) {
   EncodeTiledFn fn = get_encode_fn();
   if (!fn) return fail(SA_ERR_CUDA, "cuTensorMapEncodeTiled entry point not available");
+  const bool i8 = elem == SA_ELEM_INT8;
   cuuint64_t gdim[2] = {static_cast<cuuint64_t>(dim), rows};
-  cuuint64_t gstride[1] = {static_cast<cuuint64_t>(dim) * 2};
-  cuuint32_t box[2] = {static_cast<cuuint32_t>(sa::kBlockK), static_cast<cuuint32_t>(box_rows)};
+  cuuint64_t gstride[1] = {static_cast<cuuint64_t>(dim) * sa::elem_bytes(elem)};
+  cuuint32_t box[2] = {static_cast<cuuint32_t>(i8 ? sa::kBlockKI8 : sa::kBlockK), static_cast<cuuint32_t>(box_rows)};
   cuuint32_t estr[2] = {1, 1};
-  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), gdim, gstride, box, estr,
+  CUresult r = fn(m, i8 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), gdim, gstride, box, estr,
                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return fail(SA_ERR_CUDA, "cuTensorMapEncodeTiled failed with CUresult %d", (int)r);
@@ -121,8 +123,9 @@ struct sa_engine {
   int max_k = 0;
   int num_sms = 0;
   int sim = SA_SIM_COSINE;     // fixed at creation
+  int elem = SA_ELEM_BF16;     // fixed at creation: the element type of the rows and of the device queries
 
-  uint16_t* corpus = nullptr;  // caller-owned
+  void* corpus = nullptr;      // caller-owned [capacity][dim] of elem
   float* row_term = nullptr;   // caller-owned: 1/|c| (cosine), 1 (dotProduct), |c|^2/2 (euclidean); see sa_aux.cuh
   unsigned* cmax = nullptr;    // device scalar (float bits): upper bound on |c| over the committed rows (not cosine)
   unsigned long long* row_tags = nullptr;  // caller-owned [capacity] filter tags (sa_corpus_bind_tags), or nullptr
@@ -139,7 +142,7 @@ struct sa_engine {
   sa::FixEntry* fix_entries = nullptr;  // [kMaxLaunches * num_sms * 128] work queue of the exact fallback scan
   sa::FixQuery* fix_query = nullptr;    // [max_batch]
   int* fix_counters = nullptr;          // [0] queue length, [1] CTAs done (both zero between searches)
-  uint16_t* q_bf16 = nullptr;   // [max_batch][dim]
+  uint16_t* q_bf16 = nullptr;   // [max_batch][dim] converted queries: bf16, or int8 bytes in the same buffer
   float* q_f32 = nullptr;       // [max_batch][dim]  (host-path staging on device)
   float* res_score = nullptr;   // [max_batch][max_k]
   int* res_idx = nullptr;
@@ -315,7 +318,7 @@ struct ScanVariant {
   ScanLauncher launch;
 };
 constexpr int kProd = sa::kModeProd, kProf = sa::kModeProf, kDots = sa::kModeDots;
-constexpr int kMul = sa::kEpiMul, kSub = sa::kEpiSub, kFilt = sa::kEpiFilt, kDeep = sa::kEpiDeep;
+constexpr int kMul = sa::kEpiMul, kSub = sa::kEpiSub, kFilt = sa::kEpiFilt, kDeep = sa::kEpiDeep, kI8 = sa::kEpiI8;
 constexpr ScanVariant kScanVariants[] = {
     // production
     {1, 16, kProd, kMul, &launch_scan<1, 16, kProd, kMul>},
@@ -351,6 +354,35 @@ constexpr ScanVariant kScanVariants[] = {
     // debug dots
     {1, 16, kDots, kMul, &launch_scan<1, 16, kDots, kMul>},
     {2, 16, kDots, kMul, &launch_scan<2, 16, kDots, kMul>},
+    // int8 index: the same rows | kI8
+    {1, 16, kProd, kMul | kI8, &launch_scan<1, 16, kProd, kMul | kI8>},
+    {1, 32, kProd, kMul | kI8, &launch_scan<1, 32, kProd, kMul | kI8>},
+    {2, 16, kProd, kMul | kI8, &launch_scan<2, 16, kProd, kMul | kI8>},
+    {2, 32, kProd, kMul | kI8, &launch_scan<2, 32, kProd, kMul | kI8>},
+    {1, 16, kProd, kSub | kI8, &launch_scan<1, 16, kProd, kSub | kI8>},
+    {1, 32, kProd, kSub | kI8, &launch_scan<1, 32, kProd, kSub | kI8>},
+    {2, 16, kProd, kSub | kI8, &launch_scan<2, 16, kProd, kSub | kI8>},
+    {2, 32, kProd, kSub | kI8, &launch_scan<2, 32, kProd, kSub | kI8>},
+    {1, 16, kProd, kMul | kFilt | kI8, &launch_scan<1, 16, kProd, kMul | kFilt | kI8>},
+    {1, 32, kProd, kMul | kFilt | kI8, &launch_scan<1, 32, kProd, kMul | kFilt | kI8>},
+    {2, 16, kProd, kMul | kFilt | kI8, &launch_scan<2, 16, kProd, kMul | kFilt | kI8>},
+    {2, 32, kProd, kMul | kFilt | kI8, &launch_scan<2, 32, kProd, kMul | kFilt | kI8>},
+    {1, 16, kProd, kSub | kFilt | kI8, &launch_scan<1, 16, kProd, kSub | kFilt | kI8>},
+    {1, 32, kProd, kSub | kFilt | kI8, &launch_scan<1, 32, kProd, kSub | kFilt | kI8>},
+    {2, 16, kProd, kSub | kFilt | kI8, &launch_scan<2, 16, kProd, kSub | kFilt | kI8>},
+    {2, 32, kProd, kSub | kFilt | kI8, &launch_scan<2, 32, kProd, kSub | kFilt | kI8>},
+    {1, 32, kProd, kMul | kDeep | kI8, &launch_scan<1, 32, kProd, kMul | kDeep | kI8>},
+    {2, 32, kProd, kMul | kDeep | kI8, &launch_scan<2, 32, kProd, kMul | kDeep | kI8>},
+    {1, 32, kProd, kSub | kDeep | kI8, &launch_scan<1, 32, kProd, kSub | kDeep | kI8>},
+    {2, 32, kProd, kSub | kDeep | kI8, &launch_scan<2, 32, kProd, kSub | kDeep | kI8>},
+    {1, 32, kProd, kMul | kFilt | kDeep | kI8, &launch_scan<1, 32, kProd, kMul | kFilt | kDeep | kI8>},
+    {2, 32, kProd, kMul | kFilt | kDeep | kI8, &launch_scan<2, 32, kProd, kMul | kFilt | kDeep | kI8>},
+    {1, 32, kProd, kSub | kFilt | kDeep | kI8, &launch_scan<1, 32, kProd, kSub | kFilt | kDeep | kI8>},
+    {2, 32, kProd, kSub | kFilt | kDeep | kI8, &launch_scan<2, 32, kProd, kSub | kFilt | kDeep | kI8>},
+    {1, 16, kProf, kMul | kI8, &launch_scan<1, 16, kProf, kMul | kI8>},
+    {2, 16, kProf, kMul | kI8, &launch_scan<2, 16, kProf, kMul | kI8>},
+    {1, 16, kDots, kMul | kI8, &launch_scan<1, 16, kDots, kMul | kI8>},
+    {2, 16, kDots, kMul | kI8, &launch_scan<2, 16, kDots, kMul | kI8>},
 };
 
 int launch_scan_dispatch(int cg, int kl, int mode, int epi, const CUtensorMap& tq, const CUtensorMap& tc,
@@ -358,9 +390,9 @@ int launch_scan_dispatch(int cg, int kl, int mode, int epi, const CUtensorMap& t
   for (const ScanVariant& v : kScanVariants)
     if (v.cg == cg && v.kl == kl && v.mode == mode && v.epi == epi) return v.launch(tq, tc, p, grid, st);
   static const char* const kBuild[] = {"production", "debug-dots", "profiling"};  // indexed by sa::kMode*
-  return fail(SA_ERR_ARG, "no scan instantiation for cta_group %d, %d-entry lists, %s build, %s%s%s epilogue", cg, kl,
+  return fail(SA_ERR_ARG, "no scan instantiation for cta_group %d, %d-entry lists, %s build, %s%s%s%s epilogue", cg, kl,
               kBuild[mode], (epi & kSub) ? "subtract" : "multiply", (epi & kFilt) ? " filtered" : "",
-              (epi & kDeep) ? " deep" : "");
+              (epi & kDeep) ? " deep" : "", (epi & kI8) ? " int8" : "");
 }
 
 int choose_cg(const sa_engine* e, int nq) {
@@ -390,7 +422,13 @@ int check_engine(const sa_engine* e) {
 // (<= |q||c| by Cauchy-Schwarz): dim * 2^-23;  the inverse norm (fp32 sum of squares over dim/32 terms per lane + a
 // 5-level butterfly, one square root, one division) and the final multiply: (dim/64 + 6) * 2^-23, rounded up generously.
 // Measured worst case on adversarial inputs is ~100x smaller (tests/test_gpu_parity.py::test_scan_error_is_inside_eps).
-float scan_eps_rel(int dim) { return (1.0625f * dim + 16.0f) * 1.1920929e-07f; }
+// int8: the accumulator is the exact integer <q,c>, so only its conversion to fp32 (2^-24 |<q,c>|), the row term's one
+// rounding (2^-24) and the final multiply (2^-24) remain: 3 * 2^-24 relative (cosine), rounded up to 4 * 2^-23 whatever
+// the dim.  The euclidean subtraction and its row term are covered by cert_eps's own 2^-23 terms (DESIGN.md section 4.2).
+constexpr float kScanEpsRelI8 = 4.0f * 1.1920929e-07f;
+float scan_eps_rel(int dim, int elem) {
+  return elem == SA_ELEM_INT8 ? kScanEpsRelI8 : (1.0625f * dim + 16.0f) * 1.1920929e-07f;
+}
 
 int zero_scan_scratch(sa_engine* e, cudaStream_t st) {
   SA_CUDA(cudaMemsetAsync(e->thr_shared, 0, sizeof(unsigned) * e->thr_n, st));
@@ -416,11 +454,16 @@ int check_search(const sa_engine* e, const void* filters, bool filtered) {
   return rc;
 }
 
+// fp32 queries -> the engine's element type in the query scratch (int8: f32_to_i8, the bytes of the same buffer)
 int convert_queries(sa_engine* e, const float* q_f32_dev, int nq, cudaStream_t st) {
   SA_CUDA(cudaStreamWaitEvent(st, e->scratch_free, 0));  // q_bf16 is scratch too: the previous search still reads it
   const long long threads = static_cast<long long>(nq) * 32;
-  sa::sa_convert_rows_kernel<<<static_cast<unsigned>((threads + 255) / 256), 256, 0, st>>>(q_f32_dev, e->q_bf16,
-                                                                                         nullptr, nq, e->dim);
+  const unsigned grid = static_cast<unsigned>((threads + 255) / 256);
+  if (e->elem == SA_ELEM_INT8)
+    sa::sa_convert_rows_i8_kernel<<<grid, 256, 0, st>>>(q_f32_dev, reinterpret_cast<int8_t*>(e->q_bf16), nullptr, nq,
+                                                        e->dim, e->sim, nullptr);
+  else
+    sa::sa_convert_rows_kernel<<<grid, 256, 0, st>>>(q_f32_dev, e->q_bf16, nullptr, nq, e->dim);
   SA_CUDA(cudaGetLastError());
   return SA_OK;
 }
@@ -428,13 +471,13 @@ int convert_queries(sa_engine* e, const float* q_f32_dev, int nq, cudaStream_t s
 // One search = per scan launch {scan kernel, merge/certify kernel}, then one fixup kernel (exact fallback scan of the
 // ambiguous (query, lane) pairs -- normally none -- and conversion of the internal result to the caller's arrays).
 // filters (device, [nq]) != nullptr: a filtered search; every kernel sees only the rows that pass each query's filter.
-int do_search(sa_engine* e, const uint16_t* q_bf16, int nq, int k, float* out_score, int32_t* out_idx,
+int do_search(sa_engine* e, const void* q_dev, int nq, int k, float* out_score, int32_t* out_idx,
               double* out_score64, sa::PackedHit* out_packed, int64_t row_offset, cudaStream_t st,
               const sa::Filter* filters = nullptr) {
   if (nq <= 0 || nq > e->max_batch) return fail(SA_ERR_CAPACITY, "nq %d outside [1, max_batch %d]", nq, e->max_batch);
   if (k <= 0 || k > e->max_k) return fail(SA_ERR_ARG, "k %d outside [1, max_k %d]", k, e->max_k);
-  if (!q_bf16 || !out_score || !out_idx) return fail(SA_ERR_ARG, "null buffer");
-  if (reinterpret_cast<uintptr_t>(q_bf16) % 16) return fail(SA_ERR_ARG, "query buffer must be 16-byte aligned");
+  if (!q_dev || !out_score || !out_idx) return fail(SA_ERR_ARG, "null buffer");
+  if (reinterpret_cast<uintptr_t>(q_dev) % 16) return fail(SA_ERR_ARG, "query buffer must be 16-byte aligned");
   SA_ON_DEVICE(e->device);
 
   // 16-entry lists for k <= 16: with the certificate any k <= kKL is exact; a margin of spare entries only makes the
@@ -452,8 +495,9 @@ int do_search(sa_engine* e, const uint16_t* q_bf16, int nq, int k, float* out_sc
     return fail(SA_ERR_CAPACITY, "batch needs %zu scan launches (max %d)", plan.size(), kMaxLaunches);
   const int mode = e->opt_profile ? sa::kModeProf : sa::kModeProd;
   const int epi = (e->sim == SA_SIM_EUCLIDEAN ? sa::kEpiSub : sa::kEpiMul) | (filters != nullptr ? sa::kEpiFilt : 0) |
-                  (deep ? sa::kEpiDeep : 0);
-  const float eps_rel = scan_eps_rel(e->dim);
+                  (deep ? sa::kEpiDeep : 0) | (e->elem == SA_ELEM_INT8 ? sa::kEpiI8 : 0);
+  const float eps_rel = scan_eps_rel(e->dim, e->elem);
+  const size_t row_bytes = static_cast<size_t>(e->dim) * sa::elem_bytes(e->elem);
 
   // The candidate lists, shared thresholds and drift counters are one set of scratch buffers: a search issued on
   // another stream than the previous one must not start before that one has finished with them.
@@ -471,16 +515,16 @@ int do_search(sa_engine* e, const uint16_t* q_bf16, int nq, int k, float* out_sc
   int min_tl = sa::kMaxLanes;
   for (size_t li = 0; li < plan.size(); ++li) {
     const LaunchPlan& lp = plan[li];
-    const uint16_t* qptr = q_bf16 + static_cast<size_t>(lp.q0) * e->dim;
+    const void* qptr = static_cast<const char*>(q_dev) + lp.q0 * row_bytes;
     CUtensorMap tq;
-    int rc = encode_rows_map(&tq, qptr, static_cast<uint64_t>(lp.nq), e->dim, sa::kBlockM);
+    int rc = encode_rows_map(&tq, qptr, static_cast<uint64_t>(lp.nq), e->dim, sa::kBlockM, e->elem);
     if (rc) return rc;
 
     sa::ScanParams sp = {};
     sp.row_term = e->row_term;
     sp.n_rows = n_rows;
     sp.nq = lp.nq;
-    sp.num_kb = e->dim / sa::kBlockK;
+    sp.num_kb = static_cast<int>(row_bytes / 128);  // 128-byte K slices
     sp.num_tiles = num_tiles;
     sp.nqb = lp.nqb;
     sp.tl_count = lp.tl;
@@ -538,6 +582,7 @@ int do_search(sa_engine* e, const uint16_t* q_bf16, int nq, int k, float* out_sc
     mp.q0 = lp.q0;
     mp.eps_rel = eps_rel;
     mp.sim = e->sim;
+    mp.elem = e->elem;
     mp.cmax = e->cmax;
     mp.res64 = e->res64 + static_cast<size_t>(lp.q0) * k;
     mp.residx = e->residx + static_cast<size_t>(lp.q0) * k;
@@ -595,7 +640,7 @@ int do_search(sa_engine* e, const uint16_t* q_bf16, int nq, int k, float* out_sc
     fp.fix_query = e->fix_query;
     fp.corpus = e->corpus;
     fp.row_term = e->row_term;
-    fp.queries = q_bf16;
+    fp.queries = q_dev;
     fp.n_rows = n_rows;
     fp.num_tiles = num_tiles;
     fp.dim = e->dim;
@@ -604,6 +649,7 @@ int do_search(sa_engine* e, const uint16_t* q_bf16, int nq, int k, float* out_sc
     const int tiles_per_lane = (std::max(num_tiles, 1) + min_tl - 1) / min_tl;
     fp.chunks_per_entry = (tiles_per_lane + sa::kFixChunkTiles - 1) / sa::kFixChunkTiles;
     fp.sim = e->sim;
+    fp.elem = e->elem;
     fp.res64 = e->res64;
     fp.residx = e->residx;
     fp.out_score = out_score;
@@ -619,7 +665,8 @@ int do_search(sa_engine* e, const uint16_t* q_bf16, int nq, int k, float* out_sc
     fp.zero_c_n = e->opt_window_bound ? static_cast<int>(plan.size()) * e->num_sms * 128 : 0;
     fp.row_tags = filters != nullptr ? e->row_tags : nullptr;
     fp.filters = filters;
-    const size_t smem = static_cast<size_t>(e->dim) * sizeof(float);
+    // the query in shared memory: as fp32 (bf16), or its bytes (int8)
+    const size_t smem = e->elem == SA_ELEM_INT8 ? row_bytes : static_cast<size_t>(e->dim) * sizeof(float);
     if (smem > 48 * 1024)
       SA_CUDA(cudaFuncSetAttribute(sa::sa_fixup_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
     sa::sa_fixup_kernel<<<2 * e->num_sms, sa::kFixThreads, smem, st>>>(fp);
@@ -629,9 +676,10 @@ int do_search(sa_engine* e, const uint16_t* q_bf16, int nq, int k, float* out_sc
   }
   SA_CUDA(cudaEventRecord(tm.ev_total[1], st));
   SA_CUDA(cudaEventRecord(e->scratch_free, st));
-  // Algorithmic work (DESIGN.md section 5): corpus + inverse norms once per scan launch, queries, results.
-  const double n = static_cast<double>(n_rows), d = e->dim, b = nq;
-  tm.bytes = plan.size() * (n * d * 2.0 + n * 4.0) + b * d * 2.0 + b * k * 8.0;
+  // Algorithmic work (DESIGN.md section 5): corpus + inverse norms once per scan launch, queries, results (the rows and
+  // queries at their element size; flops are int8 ops for an int8 engine, with the same formula).
+  const double n = static_cast<double>(n_rows), d = e->dim, b = nq, es = sa::elem_bytes(e->elem);
+  tm.bytes = plan.size() * (n * d * es + n * 4.0) + b * d * es + b * k * 8.0;
   tm.flops = 2.0 * b * n * d;
   e->n_searches += 1;
   return SA_OK;
@@ -699,11 +747,21 @@ int sa_engine_create(sa_engine** out, int device, int dim, int64_t capacity_rows
 
 int sa_engine_create_sim(sa_engine** out, int device, int dim, int64_t capacity_rows, int max_batch, int max_k,
                          int similarity) {
+  return sa_engine_create_elem(out, device, dim, capacity_rows, max_batch, max_k, similarity, SA_ELEM_BF16);
+}
+
+int sa_engine_create_elem(sa_engine** out, int device, int dim, int64_t capacity_rows, int max_batch, int max_k,
+                          int similarity, int elem) {
   if (!out) return fail(SA_ERR_ARG, "null out");
   *out = nullptr;
   if (similarity != SA_SIM_COSINE && similarity != SA_SIM_DOT && similarity != SA_SIM_EUCLIDEAN)
     return fail(SA_ERR_ARG, "similarity %d is not SA_SIM_COSINE (0), SA_SIM_DOT (1) or SA_SIM_EUCLIDEAN (2)", similarity);
+  if (elem != SA_ELEM_BF16 && elem != SA_ELEM_INT8)
+    return fail(SA_ERR_ARG, "elem %d is not SA_ELEM_BF16 (0) or SA_ELEM_INT8 (1)", elem);
   if (dim <= 0 || dim % 64 != 0) return fail(SA_ERR_ARG, "dim %d must be a positive multiple of 64", dim);
+  // int8: a K slice is 128 elements, and |<q,c>| <= dim 2^14 must stay inside the int32 accumulators
+  if (elem == SA_ELEM_INT8 && (dim % 128 != 0 || dim > 65536))
+    return fail(SA_ERR_ARG, "an int8 index needs dim %d to be a multiple of 128 and at most 65536", dim);
   if (capacity_rows <= 0 || capacity_rows >= (1ll << 31) - 512)
     return fail(SA_ERR_ARG, "capacity_rows %lld outside (0, 2^31-512)", (long long)capacity_rows);
   if (max_batch <= 0) return fail(SA_ERR_ARG, "max_batch must be positive");
@@ -722,6 +780,7 @@ int sa_engine_create_sim(sa_engine** out, int device, int dim, int64_t capacity_
   sa_engine* e = new sa_engine();
   e->device = device;
   e->sim = similarity;
+  e->elem = elem;
   e->dim = dim;
   e->capacity = capacity_rows;
   e->max_batch = max_batch;
@@ -849,19 +908,19 @@ constexpr int kIngestBlock = 256;  // one warp per row
 unsigned ingest_grid(int64_t n) { return static_cast<unsigned>((n * 32 + kIngestBlock - 1) / kIngestBlock); }
 }  // namespace
 
-int sa_corpus_bind(sa_engine* e, void* rows_bf16_dev, float* row_term_dev, int64_t n_valid) {
-  if (!e || !rows_bf16_dev || !row_term_dev) return fail(SA_ERR_ARG, "null argument");
-  if (reinterpret_cast<uintptr_t>(rows_bf16_dev) % 16) return fail(SA_ERR_ARG, "corpus must be 16-byte aligned");
+int sa_corpus_bind(sa_engine* e, void* rows_dev, float* row_term_dev, int64_t n_valid) {
+  if (!e || !rows_dev || !row_term_dev) return fail(SA_ERR_ARG, "null argument");
+  if (reinterpret_cast<uintptr_t>(rows_dev) % 16) return fail(SA_ERR_ARG, "corpus must be 16-byte aligned");
   if (reinterpret_cast<uintptr_t>(row_term_dev) % 16) return fail(SA_ERR_ARG, "row_term must be 16-byte aligned");
   if (n_valid < 0 || n_valid > e->capacity) return fail(SA_ERR_CAPACITY, "n_valid outside [0, capacity]");
   SA_ON_DEVICE(e->device);
-  int rc = encode_rows_map(&e->tmap_c[0], rows_bf16_dev, static_cast<uint64_t>(e->capacity), e->dim,
-                           sa::ScanCfg<1>::kBRows);
+  int rc = encode_rows_map(&e->tmap_c[0], rows_dev, static_cast<uint64_t>(e->capacity), e->dim,
+                           sa::ScanCfg<1>::kBRows, e->elem);
   if (rc) return rc;
-  rc = encode_rows_map(&e->tmap_c[1], rows_bf16_dev, static_cast<uint64_t>(e->capacity), e->dim,
-                       sa::ScanCfg<2>::kBRows);
+  rc = encode_rows_map(&e->tmap_c[1], rows_dev, static_cast<uint64_t>(e->capacity), e->dim,
+                       sa::ScanCfg<2>::kBRows, e->elem);
   if (rc) return rc;
-  e->corpus = static_cast<uint16_t*>(rows_bf16_dev);
+  e->corpus = rows_dev;
   e->row_term = row_term_dev;
   e->n_rows = n_valid;
   e->bound = true;
@@ -869,8 +928,12 @@ int sa_corpus_bind(sa_engine* e, void* rows_bf16_dev, float* row_term_dev, int64
     // Cmax over the rows taken as committed (the legacy default stream orders this before later work on blocking streams)
     SA_CUDA(cudaMemsetAsync(e->cmax, 0, sizeof(unsigned), 0));
     if (n_valid > 0) {
-      sa::sa_rowterm_kernel<sa::kSimDot><<<ingest_grid(n_valid), kIngestBlock, 0, 0>>>(e->corpus, nullptr, -1, n_valid,
-                                                                                      e->dim, e->cmax);
+      if (e->elem == SA_ELEM_INT8)
+        sa::sa_rowterm_i8_kernel<<<ingest_grid(n_valid), kIngestBlock, 0, 0>>>(static_cast<const int8_t*>(e->corpus),
+                                                                              nullptr, -1, n_valid, e->dim, e->sim, e->cmax);
+      else
+        sa::sa_rowterm_kernel<sa::kSimDot><<<ingest_grid(n_valid), kIngestBlock, 0, 0>>>(
+            static_cast<const uint16_t*>(e->corpus), nullptr, -1, n_valid, e->dim, e->cmax);
       SA_CUDA(cudaGetLastError());
     }
   }
@@ -892,13 +955,18 @@ int sa_corpus_commit(sa_engine* e, int64_t first_row, int64_t n_new, uintptr_t s
   if (n_new == 0) return SA_OK;
   SA_ON_DEVICE(e->device);
   const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  if (e->sim == SA_SIM_COSINE)
-    sa::sa_rownorm_kernel<<<ingest_grid(n_new), kIngestBlock, 0, st>>>(e->corpus, e->row_term, first_row, n_new, e->dim);
+  const uint16_t* rows = static_cast<const uint16_t*>(e->corpus);
+  if (e->elem == SA_ELEM_INT8)
+    sa::sa_rowterm_i8_kernel<<<ingest_grid(n_new), kIngestBlock, 0, st>>>(static_cast<const int8_t*>(e->corpus),
+                                                                         e->row_term, first_row, n_new, e->dim, e->sim,
+                                                                         e->cmax);
+  else if (e->sim == SA_SIM_COSINE)
+    sa::sa_rownorm_kernel<<<ingest_grid(n_new), kIngestBlock, 0, st>>>(rows, e->row_term, first_row, n_new, e->dim);
   else if (e->sim == SA_SIM_DOT)
-    sa::sa_rowterm_kernel<sa::kSimDot><<<ingest_grid(n_new), kIngestBlock, 0, st>>>(e->corpus, e->row_term, first_row,
+    sa::sa_rowterm_kernel<sa::kSimDot><<<ingest_grid(n_new), kIngestBlock, 0, st>>>(rows, e->row_term, first_row,
                                                                                    n_new, e->dim, e->cmax);
   else
-    sa::sa_rowterm_kernel<sa::kSimEuc><<<ingest_grid(n_new), kIngestBlock, 0, st>>>(e->corpus, e->row_term, first_row,
+    sa::sa_rowterm_kernel<sa::kSimEuc><<<ingest_grid(n_new), kIngestBlock, 0, st>>>(rows, e->row_term, first_row,
                                                                                    n_new, e->dim, e->cmax);
   SA_CUDA(cudaGetLastError());
   e->n_rows = first_row + n_new;
@@ -913,9 +981,12 @@ int sa_corpus_append_f32(sa_engine* e, const float* rows_f32_dev, int64_t n_new,
   if (n_new == 0) return SA_OK;
   SA_ON_DEVICE(e->device);
   const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  uint16_t* dst = e->corpus + e->n_rows * e->dim;
   float* w = e->row_term + e->n_rows;
-  if (e->sim == SA_SIM_COSINE)
+  uint16_t* dst = static_cast<uint16_t*>(e->corpus) + e->n_rows * e->dim;
+  if (e->elem == SA_ELEM_INT8)
+    sa::sa_convert_rows_i8_kernel<<<ingest_grid(n_new), kIngestBlock, 0, st>>>(
+        rows_f32_dev, static_cast<int8_t*>(e->corpus) + e->n_rows * e->dim, w, n_new, e->dim, e->sim, e->cmax);
+  else if (e->sim == SA_SIM_COSINE)
     sa::sa_convert_rows_kernel<<<ingest_grid(n_new), kIngestBlock, 0, st>>>(rows_f32_dev, dst, w, n_new, e->dim);
   else if (e->sim == SA_SIM_DOT)
     sa::sa_convert_rows_term_kernel<sa::kSimDot><<<ingest_grid(n_new), kIngestBlock, 0, st>>>(rows_f32_dev, dst, w, n_new,
@@ -967,7 +1038,7 @@ int sa_search(sa_engine* e, const void* q_bf16_dev, int nq, int k, float* out_sc
               double* out_score64_dev, uintptr_t stream) {
   int rc = check_engine(e);
   if (rc) return rc;
-  return do_search(e, static_cast<const uint16_t*>(q_bf16_dev), nq, k, out_score_dev, out_idx_dev, out_score64_dev,
+  return do_search(e, q_bf16_dev, nq, k, out_score_dev, out_idx_dev, out_score64_dev,
                    nullptr, 0, reinterpret_cast<cudaStream_t>(stream));
 }
 
@@ -975,7 +1046,7 @@ int sa_search_filtered(sa_engine* e, const void* q_bf16_dev, const sa_filter* fi
                        float* out_score_dev, int32_t* out_idx_dev, double* out_score64_dev, uintptr_t stream) {
   int rc = check_search(e, filters_dev, true);
   if (rc) return rc;
-  return do_search(e, static_cast<const uint16_t*>(q_bf16_dev), nq, k, out_score_dev, out_idx_dev, out_score64_dev,
+  return do_search(e, q_bf16_dev, nq, k, out_score_dev, out_idx_dev, out_score64_dev,
                    nullptr, 0, reinterpret_cast<cudaStream_t>(stream), reinterpret_cast<const sa::Filter*>(filters_dev));
 }
 
@@ -1082,7 +1153,8 @@ struct sa_comm {
   std::vector<ncclComm_t> comms;    // one per local rank
   std::vector<sa::PackedHit*> gathered;  // per local rank: [n_ranks][cap_nq][cap_k], grown on demand
   std::vector<size_t> gathered_elems;
-  int sim = -1;                     // one process per GPU: the similarity every rank's engine was found to have
+  int sim = -1;                     // one process per GPU: the similarity every rank's engine was found to have ...
+  int elem = -1;                    // ... and its element type
 };
 
 namespace {
@@ -1108,12 +1180,12 @@ int comm_gather_buffer(sa_comm* c, int local, int nq, int k, sa::PackedHit** out
 // the steps (bit 0 scan, bit 1 all-gather, bit 2 merge) so a single process driving several GPUs can put the collectives
 // of all its ranks into one NCCL group (inside a group the collective is only enqueued at ncclGroupEnd, so nothing that
 // must follow it on the stream may be issued before the group closes).
-int sharded_search_on_stream(sa_comm* c, int local, sa_engine* e, const uint16_t* q_bf16, int nq, int k,
+int sharded_search_on_stream(sa_comm* c, int local, sa_engine* e, const void* q_dev, int nq, int k,
                              int64_t row_offset, float* out_score_dev, long long* out_row_dev, cudaStream_t st,
                              int phases = 7, const sa::Filter* filters = nullptr) {
   int rc;
   if (phases & 1) {
-    rc = do_search(e, q_bf16, nq, k, e->res_score, e->res_idx, nullptr, e->hits, row_offset, st, filters);
+    rc = do_search(e, q_dev, nq, k, e->res_score, e->res_idx, nullptr, e->hits, row_offset, st, filters);
     if (rc) return rc;
   }
   sa::PackedHit* gathered = nullptr;
@@ -1272,7 +1344,7 @@ static int search_hits(sa_engine* e, const void* q_bf16_dev, const sa_filter* fi
     SA_ON_DEVICE(e->device);
     SA_CUDA(cudaStreamWaitEvent(st, e->scratch_free, 0));  // res_score / res_idx below are engine scratch
   }
-  return do_search(e, static_cast<const uint16_t*>(q_bf16_dev), nq, k, e->res_score, e->res_idx, nullptr,
+  return do_search(e, q_bf16_dev, nq, k, e->res_score, e->res_idx, nullptr,
                    reinterpret_cast<sa::PackedHit*>(out_hits_dev), row_offset, st,
                    reinterpret_cast<const sa::Filter*>(filters_dev));
 }
@@ -1390,25 +1462,33 @@ int check_rank_comm(sa_comm* c, const sa_engine* e) {
   if (c->devices[0] != e->device) return fail(SA_ERR_ARG, "communicator is on device %d, engine on %d", c->devices[0], e->device);
   if (c->sim >= 0) {
     if (c->sim != e->sim) return fail(SA_ERR_ARG, "engine has similarity %d, the communicator's ranks %d", e->sim, c->sim);
+    if (c->elem != e->elem)
+      return fail(SA_ERR_ARG, "engine has element type %d, the communicator's ranks %d", e->elem, c->elem);
     return SA_OK;
   }
-  // First search on this communicator (a collective, like the search itself): all-gather every rank's similarity once;
-  // shards ranked under different similarities cannot be merged.
+  // First search on this communicator (a collective, like the search itself): all-gather every rank's (similarity,
+  // element type) once; shards ranked under different similarities, or holding other element types, cannot be merged.
   SA_ON_DEVICE(e->device);
   int* d = nullptr;
-  SA_CUDA(cudaMalloc(&d, sizeof(int) * (c->n_ranks + 1)));
-  std::vector<int> got(c->n_ranks, -1);
-  cudaError_t ce = cudaMemcpy(d + c->n_ranks, &e->sim, sizeof(int), cudaMemcpyHostToDevice);
+  SA_CUDA(cudaMalloc(&d, sizeof(int) * 2 * (c->n_ranks + 1)));
+  std::vector<int> got(2 * c->n_ranks, -1);
+  const int mine[2] = {e->sim, e->elem};
+  cudaError_t ce = cudaMemcpy(d + 2 * c->n_ranks, mine, sizeof mine, cudaMemcpyHostToDevice);
   ncclResult_t nr = ncclSuccess;
-  if (ce == cudaSuccess) nr = g_nccl.AllGather(d + c->n_ranks, d, 1, ncclInt32, c->comms[0], e->own_stream);
+  if (ce == cudaSuccess) nr = g_nccl.AllGather(d + 2 * c->n_ranks, d, 2, ncclInt32, c->comms[0], e->own_stream);
   if (ce == cudaSuccess && nr == ncclSuccess) ce = cudaStreamSynchronize(e->own_stream);
-  if (ce == cudaSuccess && nr == ncclSuccess) ce = cudaMemcpy(got.data(), d, sizeof(int) * c->n_ranks, cudaMemcpyDeviceToHost);
+  if (ce == cudaSuccess && nr == ncclSuccess)
+    ce = cudaMemcpy(got.data(), d, sizeof(int) * 2 * c->n_ranks, cudaMemcpyDeviceToHost);
   cudaFree(d);
   if (nr != ncclSuccess) return fail(SA_ERR_COMM, "similarity all-gather failed: %s", g_nccl.GetErrorString(nr));
   if (ce != cudaSuccess) return fail(SA_ERR_CUDA, "similarity all-gather: %s", cudaGetErrorString(ce));
-  for (int r = 0; r < c->n_ranks; ++r)
-    if (got[r] != e->sim) return fail(SA_ERR_ARG, "rank %d has similarity %d, this rank %d", r, got[r], e->sim);
+  for (int r = 0; r < c->n_ranks; ++r) {
+    if (got[2 * r] != e->sim) return fail(SA_ERR_ARG, "rank %d has similarity %d, this rank %d", r, got[2 * r], e->sim);
+    if (got[2 * r + 1] != e->elem)
+      return fail(SA_ERR_ARG, "rank %d has element type %d, this rank %d", r, got[2 * r + 1], e->elem);
+  }
   c->sim = e->sim;
+  c->elem = e->elem;
   return SA_OK;
 }
 }  // namespace
@@ -1424,7 +1504,7 @@ static int sharded_search(sa_comm* c, sa_engine* e, const void* q_bf16_dev, cons
   SA_ON_DEVICE(e->device);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   SA_CUDA(cudaStreamWaitEvent(st, e->scratch_free, 0));
-  return sharded_search_on_stream(c, 0, e, static_cast<const uint16_t*>(q_bf16_dev), nq, k, row_offset, out_score_dev,
+  return sharded_search_on_stream(c, 0, e, q_bf16_dev, nq, k, row_offset, out_score_dev,
                                   reinterpret_cast<long long*>(out_row_dev), st, 7,
                                   reinterpret_cast<const sa::Filter*>(filters_dev));
 }
@@ -1479,6 +1559,8 @@ static int gather_merge_submit(sa_comm* c, sa_engine* const* engines, int slot, 
       return fail(SA_ERR_ARG, "engine %d is on device %d, communicator rank %d on %d", g, engines[g]->device, g, c->devices[g]);
     if (engines[g]->sim != engines[0]->sim)
       return fail(SA_ERR_ARG, "engine %d has similarity %d, engine 0 has %d", g, engines[g]->sim, engines[0]->sim);
+    if (engines[g]->elem != engines[0]->elem)
+      return fail(SA_ERR_ARG, "engine %d has element type %d, engine 0 has %d", g, engines[g]->elem, engines[0]->elem);
     if (filters_host != nullptr) {
       rc = check_filtered(engines[g], filters_host);
       if (rc) return rc;
@@ -1665,8 +1747,10 @@ int sa_get_info(const sa_engine* e, const char* name, int64_t* value) {
   else if (!strcmp(name, "last_grid")) *value = e->last_grid;
   else if (!strcmp(name, "dbg_times_ptr")) *value = static_cast<int64_t>(reinterpret_cast<uintptr_t>(e->dbg_times));
   else if (!strcmp(name, "last_fix_entries")) *value = e->last_fix_entries;
-  else if (!strcmp(name, "eps_rel_e12")) *value = static_cast<int64_t>(static_cast<double>(scan_eps_rel(e->dim)) * 1e12);
+  else if (!strcmp(name, "eps_rel_e12"))
+    *value = static_cast<int64_t>(static_cast<double>(scan_eps_rel(e->dim, e->elem)) * 1e12);
   else if (!strcmp(name, "similarity")) *value = e->sim;
+  else if (!strcmp(name, "elem")) *value = e->elem;
   else if (!strcmp(name, "has_tags")) *value = e->row_tags != nullptr ? 1 : 0;
   else if (!strcmp(name, "cmax_bits")) {
     unsigned bits = 0;
@@ -1703,13 +1787,13 @@ int sa_debug_tile_dots(sa_engine* e, const void* q_bf16_dev, int nq, int tile, i
   if (nq <= 0 || nqb * cta_group > e->num_sms) return fail(SA_ERR_CAPACITY, "nq too large for the debug hook");
   SA_ON_DEVICE(e->device);
   CUtensorMap tq;
-  rc = encode_rows_map(&tq, q_bf16_dev, static_cast<uint64_t>(nq), e->dim, sa::kBlockM);
+  rc = encode_rows_map(&tq, q_bf16_dev, static_cast<uint64_t>(nq), e->dim, sa::kBlockM, e->elem);
   if (rc) return rc;
   sa::ScanParams sp = {};
   sp.row_term = e->row_term;
   sp.n_rows = e->n_rows;
   sp.nq = nq;
-  sp.num_kb = e->dim / sa::kBlockK;
+  sp.num_kb = e->dim * sa::elem_bytes(e->elem) / 128;  // 128-byte K slices
   sp.num_tiles = num_tiles;
   sp.nqb = nqb;
   sp.tl_count = 1;  // one tile lane: every unit walks all tiles, dumps `tile`
@@ -1719,7 +1803,8 @@ int sa_debug_tile_dots(sa_engine* e, const void* q_bf16_dev, int nq, int tile, i
   sp.tile_stride = 1;
   sp.dbg_dots = out_dots_dev;
   sp.dbg_tile = tile;
-  return launch_scan_dispatch(cta_group, 16, sa::kModeDots, sa::kEpiMul, tq, e->tmap_c[cta_group - 1], sp, nqb * cta_group,
+  const int epi = sa::kEpiMul | (e->elem == SA_ELEM_INT8 ? sa::kEpiI8 : 0);
+  return launch_scan_dispatch(cta_group, 16, sa::kModeDots, epi, tq, e->tmap_c[cta_group - 1], sp, nqb * cta_group,
                               reinterpret_cast<cudaStream_t>(stream));
 }
 
@@ -1757,6 +1842,12 @@ int sa_debug_bf16_round(const float* x, int n, uint16_t* bits, float* back) {
     bits[i] = static_cast<uint16_t>(sa::f32_to_bf16_bits(x[i]));
     back[i] = sa::bf16_bits_to_f32(bits[i]);
   }
+  return SA_OK;
+}
+
+int sa_debug_int8_round(const float* x, int n, int8_t* out) {
+  if (!x || !out || n < 0) return fail(SA_ERR_ARG, "bad argument");
+  for (int i = 0; i < n; ++i) out[i] = static_cast<int8_t>(sa::f32_to_i8(x[i]));
   return SA_OK;
 }
 

@@ -1,4 +1,4 @@
-// Kernels either side of the scan: ingest (fp32 -> bf16 + row L2 norms), candidate merge + exact
+// Kernels either side of the scan: ingest (fp32 -> bf16 or int8 + row terms), candidate merge + exact
 // rescoring, and the cross-shard merge that follows the all-gather.  All are HBM/latency-bound
 // integer/byte work on CUDA cores: coalesced 16-byte accesses, one warp per row / one block per query.
 #pragma once
@@ -46,6 +46,22 @@ __host__ __device__ __forceinline__ uint32_t f32_to_bf16_bits(float f) {
   if ((u & 0x7fffffffu) > 0x7f800000u) return (u >> 16) | 0x40u;
   return (u + 0x7fffu + ((u >> 16) & 1u)) >> 16;
 }
+// fp32 -> int8 of an int8 index (sa_debug_int8_round): round to nearest even, saturate to [-128, 127], NaN -> 0 -- the
+// rule of cvt.rni.sat.s8.f32, spelled out so that the host test hook evaluates the very same function.
+__host__ __device__ __forceinline__ int f32_to_i8(float f) {
+  if (!(f == f)) return 0;
+  f = f < -128.f ? -128.f : (f > 127.f ? 127.f : f);
+#ifdef __CUDA_ARCH__
+  return __float2int_rn(f);
+#else
+  return static_cast<int>(rintf(f));  // the host's default rounding mode: to nearest even
+#endif
+}
+__device__ __forceinline__ int warp_sum(int v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -65,6 +81,10 @@ __device__ __forceinline__ double warp_sum(double v) {
 constexpr int kSimCos = 0;
 constexpr int kSimDot = 1;
 constexpr int kSimEuc = 2;
+// Element type of an index (SA_ELEM_* of sa_api.h): rows and queries stored as bf16 or as int8.
+constexpr int kElemBf16 = 0;
+constexpr int kElemI8 = 1;
+__host__ __device__ __forceinline__ int elem_bytes(int elem) { return elem == kElemI8 ? 1 : 2; }
 
 // Row term of a live row from its float64 sum of squares (dotProduct, euclidean); cosine keeps its fp32 path below.
 // |c|^2 is summed in fp64 and rounded once: an fp32 sum of 1536 squares is off by ~1e-4 relative, the size of the whole
@@ -202,6 +222,78 @@ __global__ void sa_convert_rows_term_kernel(const float* __restrict__ src, uint1
   block_raise_cmax(cmax, &blk_max, nb, active && lane == 0);
 }
 
+// ---- int8 rows.  Sums of int8 products are exact integers (|sum| <= dim 2^14 <= 2^30 for dim <= 65536), so the sum of
+// squares is exact, and each row term is rounded once from it in fp64: 1/|c| (0 for an all-zero row), 1, or |c|^2/2.
+__device__ __forceinline__ int dp4a_s8(unsigned a, unsigned b, int c) {
+  return __dp4a(static_cast<int>(a), static_cast<int>(b), c);
+}
+__device__ __forceinline__ float row_term_i8(int sim, int ss) {
+  const double d = static_cast<double>(ss);
+  if (sim == kSimCos) return ss > 0 ? __double2float_rn(1.0 / sqrt(d)) : 0.f;
+  return sim == kSimEuc ? __double2float_rn(0.5 * d) : 1.0f;
+}
+// Exact sum of squares of one int8 row, one warp (16-byte loads, dim % 128 == 0), every lane gets it.
+__device__ __forceinline__ int row_ss_i8(const uint4* __restrict__ src, int nvec, int lane) {
+  int ss = 0;
+  for (int i = lane; i < nvec; i += 32) {
+    const uint4 x = __ldg(src + i);
+    ss = dp4a_s8(x.x, x.x, ss);
+    ss = dp4a_s8(x.y, x.y, ss);
+    ss = dp4a_s8(x.z, x.z, ss);
+    ss = dp4a_s8(x.w, x.w, ss);
+  }
+  return warp_sum(ss);
+}
+
+// Row terms of int8 rows written in place (sa_corpus_commit), Cmax raised to cover them.  first < 0: recompute Cmax only
+// (sa_corpus_bind), leaving w untouched.  One warp per row.
+__global__ void sa_rowterm_i8_kernel(const int8_t* __restrict__ rows, float* __restrict__ w_out, long long first,
+                                     long long n, int dim, int sim, unsigned* __restrict__ cmax) {
+  __shared__ unsigned blk_max;
+  const long long w = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  const bool active = w < n;
+  unsigned nb = 0u;
+  if (active) {
+    const long long r = (first < 0 ? 0 : first) + w;
+    const int ss = row_ss_i8(reinterpret_cast<const uint4*>(rows + r * dim), dim / 16, lane);
+    if (lane == 0 && first >= 0) w_out[r] = row_term_i8(sim, ss);
+    nb = norm_bound_bits(static_cast<double>(ss));
+  }
+  block_raise_cmax(cmax, &blk_max, nb, active && lane == 0);
+}
+
+// dst_i8[r][:] = f32_to_i8(src_f32[r][:]).  Rows (w_out != nullptr): also the row term and Cmax, as
+// sa_rowterm_i8_kernel; queries (w_out == nullptr): the conversion only.  One warp per row, 16-byte loads.
+__global__ void sa_convert_rows_i8_kernel(const float* __restrict__ src, int8_t* __restrict__ dst, float* __restrict__ w_out,
+                                          long long n, int dim, int sim, unsigned* __restrict__ cmax) {
+  __shared__ unsigned blk_max;
+  const long long w = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  const bool active = w < n;
+  unsigned nb = 0u;
+  if (active) {
+    const float4* s = reinterpret_cast<const float4*>(src + w * dim);
+    unsigned* d = reinterpret_cast<unsigned*>(dst + w * dim);
+    int ss = 0;
+    for (int i = lane; i < dim / 4; i += 32) {
+      const float4 x = __ldg(s + i);
+      const unsigned b = (static_cast<unsigned>(f32_to_i8(x.x)) & 0xffu) |
+                         ((static_cast<unsigned>(f32_to_i8(x.y)) & 0xffu) << 8) |
+                         ((static_cast<unsigned>(f32_to_i8(x.z)) & 0xffu) << 16) |
+                         (static_cast<unsigned>(f32_to_i8(x.w)) << 24);
+      d[i] = b;
+      ss = dp4a_s8(b, b, ss);
+    }
+    ss = warp_sum(ss);
+    if (w_out != nullptr) {
+      if (lane == 0) w_out[w] = row_term_i8(sim, ss);
+      nb = norm_bound_bits(static_cast<double>(ss));
+    }
+  }
+  if (w_out != nullptr) block_raise_cmax(cmax, &blk_max, nb, active && lane == 0);  // w_out is uniform over the grid
+}
+
 // Per-query filter over the rows' 64-bit tags (sa_filter of sa_api.h, same layout).  One definition of the predicate
 // serves the scan's epilogue, the exact fallback scan and the host test hook (sa_debug_filter_pass).
 struct Filter {
@@ -251,8 +343,8 @@ struct MergeParams {
   const float* part_score;  // [grid CTAs][128][kKL] from the scan
   const int* part_idx;
   const float* part_drop;   // [grid CTAs][128]
-  const uint16_t* corpus;   // [capacity][dim] bf16
-  const uint16_t* queries;  // [nq][dim] bf16 (this launch's queries)
+  const void* corpus;       // [capacity][dim] bf16 or int8 (elem)
+  const void* queries;      // [nq][dim] bf16 or int8 (this launch's queries)
   int dim;
   int nq;
   int k;
@@ -263,6 +355,7 @@ struct MergeParams {
   int q0;                   // index of this launch's first query within the whole search
   float eps_rel;            // relative accumulation bound of the scan (cert_eps)
   int sim;                  // kSimCos / kSimDot / kSimEuc
+  int elem;                 // kElemBf16 / kElemI8
   const unsigned* cmax;     // device scalar (float bits): upper bound on |c| over the committed rows (not cosine)
   double* res64;            // [nq][k] this launch's slice of the search's internal result: value (float64) ...
   int* residx;              // ... and shard-local row, -1 / -inf when fewer than k rows qualify
@@ -283,15 +376,40 @@ __device__ __forceinline__ float key_score(unsigned long long k) {
   return key_to_float(static_cast<unsigned>(k >> 32));
 }
 
+// The internal value from the exact sums <q,c>, |c|^2 and |q|^2 (the one formula of every element type).
+__device__ __forceinline__ double exact_value_from_sums(double dot, double dd, double qq, int sim) {
+  if (sim == kSimDot) return dot;
+  if (sim == kSimEuc) {
+    const double d2 = __dadd_rn(__dsub_rn(qq, 2.0 * dot), dd);  // no contraction: the oracle evaluates the same two ops
+    return -sqrt(d2 > 0.0 ? d2 : 0.0);
+  }
+  const double den = qq * dd;
+  return den > 0.0 ? dot / sqrt(den) : 0.0;
+}
+
 // Exact internal value of (query, corpus row), one warp: bf16 x bf16 products are exact in fp32; sums of products and of
 // squares in float64, lane-strided then a butterfly.  Every lane returns the same value.  Used by the merge kernel AND
 // the fallback scan, so the two produce bit-identical values for the same pair.  Larger is better:
 //   cosine      <q,c> / sqrt(|q|^2 |c|^2)   (0 when either is all-zero)
 //   dotProduct  <q,c>
 //   euclidean   -sqrt(max(d2, 0)),  d2 = (|q|^2 - 2 <q,c>) + |c|^2   -- one fixed formula, the oracle's too
+// int8 (elem == kElemI8): the sums are exact int32 sums (dp4a), converted to float64 exactly; the formulas are the same.
+// nvec = 16-byte vectors per row (dim / 8 bf16, dim / 16 int8).
 __device__ __forceinline__ double exact_value_warp(const uint4* __restrict__ qv, const uint4* __restrict__ cv, int nvec,
-                                                   double qq, int lane, int sim) {
+                                                   double qq, int lane, int sim, int elem) {
   double dot = 0.0, dd = 0.0;
+  if (elem == kElemI8) {
+    int idot = 0, idd = 0;
+    for (int i = lane; i < nvec; i += 32) {
+      const uint4 x = __ldg(qv + i);
+      const uint4 y = __ldg(cv + i);
+      idot = dp4a_s8(x.x, y.x, dp4a_s8(x.y, y.y, dp4a_s8(x.z, y.z, dp4a_s8(x.w, y.w, idot))));
+      idd = dp4a_s8(y.x, y.x, dp4a_s8(y.y, y.y, dp4a_s8(y.z, y.z, dp4a_s8(y.w, y.w, idd))));
+    }
+    dot = static_cast<double>(warp_sum(idot));
+    dd = static_cast<double>(warp_sum(idd));
+    return exact_value_from_sums(dot, dd, qq, sim);
+  }
   for (int i = lane; i < nvec; i += 32) {
     const uint4 x = __ldg(qv + i);
     const uint4 y = __ldg(cv + i);
@@ -310,12 +428,7 @@ __device__ __forceinline__ double exact_value_warp(const uint4* __restrict__ qv,
   dot = warp_sum(dot);
   if (sim == kSimDot) return dot;
   dd = warp_sum(dd);
-  if (sim == kSimEuc) {
-    const double d2 = __dadd_rn(__dsub_rn(qq, 2.0 * dot), dd);  // no contraction: the oracle evaluates the same two ops
-    return -sqrt(d2 > 0.0 ? d2 : 0.0);
-  }
-  const double den = qq * dd;
-  return den > 0.0 ? dot / sqrt(den) : 0.0;
+  return exact_value_from_sums(dot, dd, qq, sim);
 }
 
 // The certificate's bound eps >= |a(r) - e(r)| for every committed row r, rounded up (DESIGN.md section 4.2).
@@ -340,7 +453,8 @@ __device__ __forceinline__ float value_to_scan_rd(int sim, double v, double qq) 
   if (sim == kSimDot) return __double2float_rd(v);
   return __double2float_rd(0.5 * (qq - v * v));  // v = -d: (|q|^2 - d^2) / 2
 }
-__device__ __forceinline__ double query_norm2_warp(const uint4* __restrict__ qv, int nvec, int lane) {
+__device__ __forceinline__ double query_norm2_warp(const uint4* __restrict__ qv, int nvec, int lane, int elem) {
+  if (elem == kElemI8) return static_cast<double>(row_ss_i8(qv, nvec, lane));  // exact
   double qq = 0.0;
   for (int i = lane; i < nvec; i += 32) {
     const uint4 x = __ldg(qv + i);
@@ -395,10 +509,11 @@ __global__ void __launch_bounds__(kMergeThreads) sa_merge_rescore_kernel(const M
     nsel_s = 0;
     namb_s = 0;
   }
-  const uint4* qv = reinterpret_cast<const uint4*>(p.queries + static_cast<size_t>(q) * p.dim);
-  const int nvec = p.dim / 8;
+  const size_t row_bytes = static_cast<size_t>(p.dim) * elem_bytes(p.elem);
+  const uint4* qv = reinterpret_cast<const uint4*>(static_cast<const char*>(p.queries) + q * row_bytes);
+  const int nvec = static_cast<int>(row_bytes / 16);
   if (warp == kMergeWarps - 1) {
-    const double qq = query_norm2_warp(qv, nvec, lane);
+    const double qq = query_norm2_warp(qv, nvec, lane, p.elem);
     if (lane == 0) qq_s = qq;
   }
   __syncthreads();
@@ -460,8 +575,8 @@ __global__ void __launch_bounds__(kMergeThreads) sa_merge_rescore_kernel(const M
   // ---- exact re-scoring: warp w takes candidates w, w + kMergeWarps, ...
   for (int c = warp; c < nsel; c += kMergeWarps) {
     const int crow = key_row(sel[c]);
-    const uint4* cv = reinterpret_cast<const uint4*>(p.corpus + static_cast<size_t>(crow) * p.dim);
-    const double v = exact_value_warp(qv, cv, nvec, qq, lane, p.sim);
+    const uint4* cv = reinterpret_cast<const uint4*>(static_cast<const char*>(p.corpus) + crow * row_bytes);
+    const double v = exact_value_warp(qv, cv, nvec, qq, lane, p.sim, p.elem);
     if (lane == 0) cs[c] = v;
   }
   __syncthreads();
@@ -523,9 +638,9 @@ struct FixParams {
   int* fix_count;
   int* done_count;
   FixQuery* fix_query;
-  const uint16_t* corpus;
+  const void* corpus;       // bf16 or int8 (elem)
   const float* row_term;
-  const uint16_t* queries;  // [nq][dim] the whole search
+  const void* queries;      // [nq][dim] the whole search
   long long n_rows;
   int num_tiles;
   int dim;
@@ -533,6 +648,7 @@ struct FixParams {
   int k;
   int chunks_per_entry;     // ceil(max tiles per lane / kFixChunkTiles)
   int sim;                  // kSimCos / kSimDot / kSimEuc
+  int elem;                 // kElemBf16 / kElemI8
   double* res64;            // [nq][k] internal result (read / updated here)
   int* residx;
   // finalisation: the internal value becomes the returned one (euclidean: the distance, -v)
@@ -594,7 +710,8 @@ __device__ __forceinline__ void fix_list_insert(D* cosv, I* rowv, int k, double 
 }
 
 __global__ void __launch_bounds__(kFixThreads) sa_fixup_kernel(const FixParams p) {
-  extern __shared__ float4 fix_smem[];  // query as fp32: [dim/8] float4 "lo" halves, then [dim/8] "hi" halves
+  extern __shared__ float4 fix_smem[];  // bf16 query as fp32: [dim/8] float4 "lo" halves, then [dim/8] "hi" halves;
+                                        // int8 query: its dim bytes as they are
   constexpr int kWarps = kFixThreads / 32;
   __shared__ double l_cos[kWarps][kFixMaxK];  // one list per warp, touched by that warp's lane 0 only
   __shared__ int l_row[kWarps][kFixMaxK];
@@ -608,9 +725,12 @@ __global__ void __launch_bounds__(kFixThreads) sa_fixup_kernel(const FixParams p
     return;
   }
 
-  const int nvec = p.dim / 8;
+  const bool i8 = p.elem == kElemI8;
+  const size_t row_bytes = static_cast<size_t>(p.dim) * elem_bytes(p.elem);
+  const int nvec = static_cast<int>(row_bytes / 16);
   float4* q_lo = fix_smem;
   float4* q_hi = fix_smem + nvec;
+  const uint4* q_i8 = reinterpret_cast<const uint4*>(fix_smem);
   const long long items = static_cast<long long>(count) * p.chunks_per_entry;
   for (long long item = blockIdx.x; item < items; item += gridDim.x) {
     const FixEntry en = p.entries[item / p.chunks_per_entry];
@@ -623,13 +743,17 @@ __global__ void __launch_bounds__(kFixThreads) sa_fixup_kernel(const FixParams p
     const float eps = fq->eps;
     volatile double* g_cos = p.res64 + static_cast<size_t>(en.q) * p.k;
     volatile int* g_row = p.residx + static_cast<size_t>(en.q) * p.k;
-    const uint4* qv = reinterpret_cast<const uint4*>(p.queries + static_cast<size_t>(en.q) * p.dim);
+    const uint4* qv = reinterpret_cast<const uint4*>(static_cast<const char*>(p.queries) + en.q * row_bytes);
     Filter flt = {0ull, 0ull, {0ull, 0ull}};  // match-all unless the search is filtered
     if (p.filters != nullptr) flt = p.filters[en.q];
 
     __syncthreads();  // previous item's smem no longer in use
     for (int i = tid; i < nvec; i += kFixThreads) {
       const uint4 x = __ldg(qv + i);
+      if (i8) {
+        reinterpret_cast<uint4*>(fix_smem)[i] = x;
+        continue;
+      }
       q_lo[i] = make_float4(bf16_bits_to_f32(x.x & 0xffffu), bf16_bits_to_f32(x.x >> 16), bf16_bits_to_f32(x.y & 0xffffu),
                             bf16_bits_to_f32(x.y >> 16));
       q_hi[i] = make_float4(bf16_bits_to_f32(x.z & 0xffffu), bf16_bits_to_f32(x.z >> 16), bf16_bits_to_f32(x.w & 0xffffu),
@@ -660,24 +784,36 @@ __global__ void __launch_bounds__(kFixThreads) sa_fixup_kernel(const FixParams p
         const float wr = __ldg(p.row_term + r);
         if (p.sim == kSimEuc ? !(wr >= 0.f) : !(wr > 0.f)) continue;  // rows that are not live are never returned
         if (p.filters != nullptr && !filter_pass(__ldg(p.row_tags + r), flt)) continue;  // nor rows the filter excludes
-        const uint4* cv = reinterpret_cast<const uint4*>(p.corpus + static_cast<size_t>(r) * p.dim);
-        float acc = 0.f;
-        for (int i = lane; i < nvec; i += 32) {
-          const uint4 y = __ldg(cv + i);
-          const float4 a = q_lo[i], b = q_hi[i];
-          acc = fmaf(a.x, bf16_bits_to_f32(y.x & 0xffffu), acc);
-          acc = fmaf(a.y, bf16_bits_to_f32(y.x >> 16), acc);
-          acc = fmaf(a.z, bf16_bits_to_f32(y.y & 0xffffu), acc);
-          acc = fmaf(a.w, bf16_bits_to_f32(y.y >> 16), acc);
-          acc = fmaf(b.x, bf16_bits_to_f32(y.z & 0xffffu), acc);
-          acc = fmaf(b.y, bf16_bits_to_f32(y.z >> 16), acc);
-          acc = fmaf(b.z, bf16_bits_to_f32(y.w & 0xffffu), acc);
-          acc = fmaf(b.w, bf16_bits_to_f32(y.w >> 16), acc);
+        const uint4* cv = reinterpret_cast<const uint4*>(static_cast<const char*>(p.corpus) + r * row_bytes);
+        float acc;
+        if (i8) {
+          // exact int32 dot (dp4a), rounded once to fp32: the scan's accumulator exactly, so a' below is the scan's a
+          int iacc = 0;
+          for (int i = lane; i < nvec; i += 32) {
+            const uint4 y = __ldg(cv + i);
+            const uint4 x = q_i8[i];
+            iacc = dp4a_s8(x.x, y.x, dp4a_s8(x.y, y.y, dp4a_s8(x.z, y.z, dp4a_s8(x.w, y.w, iacc))));
+          }
+          acc = __int2float_rn(warp_sum(iacc));
+        } else {
+          acc = 0.f;
+          for (int i = lane; i < nvec; i += 32) {
+            const uint4 y = __ldg(cv + i);
+            const float4 a = q_lo[i], b = q_hi[i];
+            acc = fmaf(a.x, bf16_bits_to_f32(y.x & 0xffffu), acc);
+            acc = fmaf(a.y, bf16_bits_to_f32(y.x >> 16), acc);
+            acc = fmaf(a.z, bf16_bits_to_f32(y.y & 0xffffu), acc);
+            acc = fmaf(a.w, bf16_bits_to_f32(y.y >> 16), acc);
+            acc = fmaf(b.x, bf16_bits_to_f32(y.z & 0xffffu), acc);
+            acc = fmaf(b.y, bf16_bits_to_f32(y.z >> 16), acc);
+            acc = fmaf(b.z, bf16_bits_to_f32(y.w & 0xffffu), acc);
+            acc = fmaf(b.w, bf16_bits_to_f32(y.w >> 16), acc);
+          }
+          acc = warp_sum(acc);
         }
-        acc = warp_sum(acc);
         const float ap = p.sim == kSimEuc ? acc - wr : acc * wr;
         if (!(ap >= thr)) continue;  // warp-uniform (every lane holds the same sum)
-        const double c = exact_value_warp(qv, cv, nvec, qq, lane, p.sim);
+        const double c = exact_value_warp(qv, cv, nvec, qq, lane, p.sim, p.elem);
         float nt = thr;
         if (lane == 0) {
           fix_list_insert(wc, wrow, p.k, c, static_cast<int>(r));

@@ -15,6 +15,9 @@
 // term becomes NaN, exactly like a tombstone's, so an ineligible row never enters a list, raises `drop` or a threshold.
 // A deep search (kEpi | kEpiDeep, 28 < k <= 64) keeps the 32-entry lists and changes only the bounds the lanes share
 // (kEpiDeep below).
+// An int8 index (kEpi | kEpiI8) multiplies int8 rows and queries with s8 wgmma into exact int32 accumulators; a K slice is
+// then 128 elements (the same 128 bytes), and the staging buffer receives the accumulators converted to fp32.  From the
+// staging buffer on, everything is the bf16 path's.
 //
 // Nothing but the per-CTA candidate lists (kKL entries per query, plus one "dropped" bound per query) leaves the SM.
 //
@@ -34,6 +37,7 @@
 #include "sa_aux.cuh"
 #include "sm90_ptx.cuh"
 #include <cmath>
+#include <type_traits>
 
 namespace sa {
 
@@ -41,6 +45,7 @@ constexpr int kBlockM = 128;  // queries per CTA
 constexpr int kBlockN = 256;  // corpus rows per tile
 constexpr int kHalfN = kWgmmaN;  // corpus rows per MMA: a tile is multiplied as two halves, each into its own accumulators
 constexpr int kBlockK = 64;   // bf16 per K slice = 128 B = one swizzle atom
+constexpr int kBlockKI8 = 128;  // int8 per K slice: the same 128 B
 constexpr int kUmmaK = 16;
 constexpr int kScanThreads = 384;  // warpgroup 0: w0 TMA producer; warpgroups 1, 2: 64 queries each (MMA + epilogue)
 // Registers per thread after the roles split (setmaxnreg): 128 x 40 + 256 x 232 = 384 x 168, the launch's allocation.
@@ -61,6 +66,10 @@ constexpr int kEpiMul = 0;     // v = acc * w; a row is live iff w > 0 (cosine, 
 constexpr int kEpiSub = 1;     // v = acc - w; a row is live iff w >= 0 (euclidean)
 constexpr int kEpiFilt = 2;    // flag: filtered search (ScanParams::row_tags / filters)
 constexpr int kEpiDeep = 4;    // flag: deep search (28 < k <= 64 with kKL = 32 entries): bounds valid for the k-th best
+constexpr int kEpiI8 = 8;      // flag: int8 rows and queries (s8 wgmma, exact int32 accumulators)
+// The int8 K slice occupies the bf16 slice's bytes, so ScanCfg (stage sizes, TMA boxes in bytes, descriptors, staging,
+// smem layout) serves both element types unchanged.
+static_assert(kBlockKI8 * 1 == kBlockK * 2, "an int8 K slice is one 128-byte swizzle atom, like a bf16 one");
 
 // Deep search.  The list, drop and masking rules are those of every search; only the bounds the lanes share change, since
 // a lane's kKL-th best says nothing about a query's k-th best once k > kKL:
@@ -112,7 +121,7 @@ struct ScanParams {
                           // tombstone; see kEpi for the others); 16-byte aligned
   long long n_rows;       // committed rows (epoch snapshot); rows >= n_rows are masked
   int nq;                 // queries covered by tmap_q
-  int num_kb;             // D / 64
+  int num_kb;             // K slices: D / 64 (int8: D / 128)
   int num_tiles;          // ceil(n_rows / 256)
   int nqb;                // query blocks of 128*kCG rows
   int tl_count;           // tile lanes (TL)
@@ -374,6 +383,9 @@ sa_scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant
                const ScanParams p) {
   constexpr bool kFilt = (kEpi & kEpiFilt) != 0;
   constexpr bool kDeep = (kEpi & kEpiDeep) != 0;
+  constexpr bool kI8 = (kEpi & kEpiI8) != 0;
+  constexpr int kSliceK = kI8 ? kBlockKI8 : kBlockK;  // elements per K slice (the TMA box's x extent)
+  using Acc = typename std::conditional<kI8, int, float>::type;
   static_assert(!kDeep || (kKL == 32 && kMode == kModeProd), "deep search: 32-entry lists, production build only");
   using Cfg = ScanCfg<kCG, kFilt>;
   static_assert(!(kDeep && kFilt) || Cfg::kSmemBytes == 228400, "the filtered deep scan has its twin's smem layout");
@@ -479,12 +491,12 @@ sa_scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant
             }
           }
           mbar_expect_tx(full_bar(stage), Cfg::kStageBytes);
-          tma_load_2d(a_smem(stage), &tmap_q, full_bar(stage), kb * kBlockK, q_row, kEvictLast);
+          tma_load_2d(a_smem(stage), &tmap_q, full_bar(stage), kb * kSliceK, q_row, kEvictLast);
           const uint32_t b_dst = b_smem(stage) + rank * (Cfg::kBRows * kBlockK * 2);
           if constexpr (kCG == 1)
-            tma_load_2d(b_dst, &tmap_c, full_bar(stage), kb * kBlockK, c_row, c_hint);
+            tma_load_2d(b_dst, &tmap_c, full_bar(stage), kb * kSliceK, c_row, c_hint);
           else
-            tma_load_2d_multicast(b_dst, &tmap_c, full_bar(stage), kb * kBlockK, c_row, 0x3, c_hint);
+            tma_load_2d_multicast(b_dst, &tmap_c, full_bar(stage), kb * kSliceK, c_row, 0x3, c_hint);
           if (++stage == kStages) {
             stage = 0;
             phase ^= 1u;
@@ -611,7 +623,7 @@ sa_scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant
       // ---- MMA: acc0 = Q[64 x D] . C[rows 0..127 of the tile]^T, acc1 the same for rows 128..255, K slice by K slice,
       // both from the same A slice; a slot is released once the MMAs reading it have retired (wait_group 1 after the
       // next slice's issue keeps one slice in flight)
-      float acc0[64], acc1[64];  // dead between tiles: the first MMA of a tile overwrites them
+      Acc acc0[64], acc1[64];  // dead between tiles: the first MMA of a tile overwrites them
       int prev_stage = -1;
       for (int kb = 0; kb < p.num_kb; ++kb) {
         if constexpr (kProf) {
@@ -626,11 +638,16 @@ sa_scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant
         wgmma_fence_operands(acc1);
 #pragma unroll
         for (int k = 0; k < kBlockK / kUmmaK; ++k) {
-          // +32 B along K inside the 128-B swizzle atom = +2 in the (addr >> 4) field
+          // +32 B along K inside the 128-B swizzle atom (16 bf16 or 32 int8) = +2 in the (addr >> 4) field
           const uint64_t a_desc = a_desc0 + stage * kStageDesc + 2u * k;
           const uint64_t b_desc = b_desc0 + stage * kStageDesc + 2u * k;
-          wgmma_m64n128k16_bf16(acc0, a_desc, b_desc, (kb | k) != 0 ? 1u : 0u);
-          wgmma_m64n128k16_bf16(acc1, a_desc, b_desc + kHalfBDesc, (kb | k) != 0 ? 1u : 0u);
+          if constexpr (kI8) {
+            wgmma_m64n128k32_s8(acc0, a_desc, b_desc, (kb | k) != 0 ? 1u : 0u);
+            wgmma_m64n128k32_s8(acc1, a_desc, b_desc + kHalfBDesc, (kb | k) != 0 ? 1u : 0u);
+          } else {
+            wgmma_m64n128k16_bf16(acc0, a_desc, b_desc, (kb | k) != 0 ? 1u : 0u);
+            wgmma_m64n128k16_bf16(acc1, a_desc, b_desc + kHalfBDesc, (kb | k) != 0 ? 1u : 0u);
+          }
         }
         wgmma_commit();
         wgmma_fence_operands(acc0);
@@ -661,7 +678,14 @@ sa_scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant
       // prefetch the next tile's row terms: issued after the MMAs, so that they hold no registers across them
       if (epi && ti + TL < walk_tiles) fetch_ic((ti + TL) * p.tile_stride);
       // ---- one half at a time through the staging buffer, rows in ascending order
-      auto stage_and_score = [&](const float (&acc)[64], int h) {
+      // int8: the exact int32 accumulator rounded once to fp32 (the scan's only accumulation error)
+      auto to_f32 = [](Acc x) {
+        if constexpr (kI8)
+          return __int2float_rn(x);
+        else
+          return x;
+      };
+      auto stage_and_score = [&](const Acc (&acc)[64], int h) {
         long long c1 = 0;
         if constexpr (kProf) c1 = clock64();
         named_bar_sync(named_bar, 128);  // the previous half's readers are done with the buffer
@@ -669,8 +693,10 @@ sa_scan_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant
         for (int j = 0; j < 16; ++j) {
           const int r = 16 * (wt >> 5) + ((wt & 31) >> 2);
           const int col = 8 * j + 2 * (wt & 3);
-          *reinterpret_cast<float2*>(stg + r * kStagingLd + col) = make_float2(acc[4 * j + 0], acc[4 * j + 1]);
-          *reinterpret_cast<float2*>(stg + (r + 8) * kStagingLd + col) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+          *reinterpret_cast<float2*>(stg + r * kStagingLd + col) =
+              make_float2(to_f32(acc[4 * j + 0]), to_f32(acc[4 * j + 1]));
+          *reinterpret_cast<float2*>(stg + (r + 8) * kStagingLd + col) =
+              make_float2(to_f32(acc[4 * j + 2]), to_f32(acc[4 * j + 3]));
         }
         named_bar_sync(named_bar, 128);
         long long c2 = 0;

@@ -208,16 +208,45 @@ __device__ __forceinline__ void wgmma_m64n128k16_bf16(float (&d)[64], uint64_t a
       : "l"(a_desc), "l"(b_desc), "r"(accumulate)
       : "memory");
 }
+// D[64 x 128] (+)= A[64 x 32] * B[128 x 32]^T from shared memory; s8 inputs, exact s32 accumulate, both K-major.  32 int8
+// elements are the 32 bytes of one bf16 k16 step, so the descriptors advance exactly as for wgmma_m64n128k16_bf16, and
+// d[] has the same (row, column) layout.
+__device__ __forceinline__ void wgmma_m64n128k32_s8(int (&d)[64], uint64_t a_desc, uint64_t b_desc,
+                                                    uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k32.s32.s8.s8 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p;\n\t}"
+      : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]),
+        "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]),
+        "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]),
+        "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]),
+        "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]),
+        "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]),
+        "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]),
+        "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63])
+      : "l"(a_desc), "l"(b_desc), "r"(accumulate)
+      : "memory");
+}
 // Keeps the compiler from moving reads or writes of the accumulators across a wgmma fence / wait.
 __device__ __forceinline__ void wgmma_fence_operands(float (&d)[64]) {
 #pragma unroll
   for (int i = 0; i < 64; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
+__device__ __forceinline__ void wgmma_fence_operands(int (&d)[64]) {
+#pragma unroll
+  for (int i = 0; i < 64; ++i) asm volatile("" : "+r"(d[i])::"memory");
+}
 
 // ----------------------------------------------------------------------------------------------
 // Descriptors
 // ----------------------------------------------------------------------------------------------
-// Shared-memory matrix descriptor for a K-major operand tile stored as TMA SWIZZLE_128B rows of 64 bf16
+// Shared-memory matrix descriptor for a K-major operand tile stored as TMA SWIZZLE_128B rows of 64 bf16 or 128 int8
 // (128 B): rows are 128 B apart, 8-row groups 1024 B apart, tile base 1024-B aligned (base offset 0).
 //   [0,14)  start address >> 4      [16,30) leading-dim byte offset >> 4 (unused for swizzled K-major, =1)
 //   [32,46) stride-dim byte offset >> 4 (1024 B between 8-row groups = 64)

@@ -74,6 +74,20 @@ def host_buffers(out, nq: int, k: int, idx_dtype=np.int32):
     return score, idx
 
 
+def int8_round(x) -> np.ndarray:
+    """fp32 -> int8 by the rule every int8 index applies to float input (sa_debug_int8_round): round to nearest even,
+    saturate to [-128, 127], NaN -> 0."""
+    x = np.ascontiguousarray(x, dtype=np.float32)
+    out = np.empty(x.shape, np.int8)
+    lib = capi.load()
+    capi.check(lib.sa_debug_int8_round(x.ctypes.data, x.size, out.ctypes.data), "sa_debug_int8_round")
+    return out
+
+
+# an index's dtype -> the torch dtype of its rows and of its device queries
+TORCH_DTYPES = {"bfloat16": torch.bfloat16, "int8": torch.int8}
+
+
 def pinned_array(shape, dtype=np.float32) -> np.ndarray:
     """A page-locked numpy array (sa_host_alloc), freed (sa_host_free) when its last view is garbage-collected."""
     import weakref
@@ -87,7 +101,13 @@ def pinned_array(shape, dtype=np.float32) -> np.ndarray:
 
 
 class VectorIndex:
-    """A row shard of the corpus resident in HBM: bf16 rows [capacity, dim] + one fp32 row term per row [capacity].
+    """A row shard of the corpus resident in HBM: bf16 (or int8) rows [capacity, dim] + one fp32 row term per row
+    [capacity].
+
+    ``dtype`` is the element type, fixed at creation: "bfloat16" (default) or "int8" (include/sa_api.h, SA_ELEM_*).  An
+    int8 index stores ``rows`` as int8, searches int8 (or fp32) queries and evaluates the similarity on the integers
+    themselves, exactly; fp32 input is rounded to nearest even and saturated to [-128, 127] (``int8_round``).  Its
+    ``dim`` must be a multiple of 128.
 
     ``similarity`` is the Atlas index setting, fixed at creation: "cosine" (default), "dotProduct" or "euclidean"
     (include/sa_api.h, SA_SIM_*).  Scores are cosines, dot products or Euclidean distances accordingly; results are
@@ -101,22 +121,24 @@ class VectorIndex:
     argument restricts each query to the rows whose tag passes its filter (``filter_array``, qsa_b200.filters)."""
 
     def __init__(self, dim: int = 1536, capacity: int = 1 << 20, max_batch: int = 1024, max_k: int = 10,
-                 device: int | None = None, similarity: str = "cosine"):
+                 device: int | None = None, similarity: str = "cosine", dtype: str = "bfloat16"):
         sim = capi.similarity_code(similarity)
+        elem = capi.elem_code(dtype)
         if not torch.cuda.is_available():
             raise RuntimeError("VectorIndex needs a CUDA device (H100, sm_90a); there is no CPU fallback")
         self.similarity = similarity
+        self.dtype = dtype
         self.lib = capi.load()
         self.device = torch.cuda.current_device() if device is None else int(device)
         self.dim, self.capacity, self.max_batch, self.max_k = int(dim), int(capacity), int(max_batch), int(max_k)
         dev = torch.device("cuda", self.device)
         # device-memory holders (the engine never copies or frees these)
-        self.rows = torch.empty((self.capacity, self.dim), dtype=torch.bfloat16, device=dev)
+        self.rows = torch.empty((self.capacity, self.dim), dtype=TORCH_DTYPES[dtype], device=dev)
         self.inv_norm = torch.zeros((self.capacity,), dtype=torch.float32, device=dev)
         self.tags = torch.zeros((self.capacity,), dtype=torch.int64, device=dev)
         h = C.c_void_p()
-        capi.check(self.lib.sa_engine_create_sim(C.byref(h), self.device, self.dim, self.capacity, self.max_batch,
-                                                 self.max_k, sim), "sa_engine_create_sim")
+        capi.check(self.lib.sa_engine_create_elem(C.byref(h), self.device, self.dim, self.capacity, self.max_batch,
+                                                  self.max_k, sim, elem), "sa_engine_create_elem")
         self._h = h
         self._inflight = {}
         capi.check(self.lib.sa_corpus_bind(self._h, self.rows.data_ptr(), self.inv_norm.data_ptr(), 0),
@@ -179,9 +201,13 @@ class VectorIndex:
         self.tags[ix] = torch.from_numpy(t.view(np.int64)).to(self.tags.device)
 
     def append(self, rows_f32, tags=None) -> int:
-        """Append fp32 embeddings (host numpy or device tensor) -> bf16 rows + norms.  Returns first row id.
+        """Append fp32 embeddings (host numpy or device tensor) -> bf16 (or int8) rows + row terms.  Returns first row
+        id.  An int8 index also takes int8 rows (numpy or CUDA tensor), stored exactly as given.
         ``tags`` (uint64 [n]) are the new rows' filter tags; without them the rows get tag 0."""
         first = len(self)
+        is_t = isinstance(rows_f32, torch.Tensor)
+        if self.dtype == "int8" and (rows_f32.dtype == torch.int8 if is_t else np.asarray(rows_f32).dtype == np.int8):
+            return self._append_in_place(rows_f32, tags)
         if isinstance(rows_f32, torch.Tensor) and rows_f32.is_cuda:
             x = rows_f32.to(torch.float32).contiguous()
             assert x.dim() == 2 and x.shape[1] == self.dim
@@ -200,14 +226,20 @@ class VectorIndex:
 
     def append_bf16_bits(self, bits: np.ndarray, tags=None) -> int:
         """Append rows given as bf16 bit patterns (uint16 [n, dim]) -- used with the synthetic corpora so the
-        device holds exactly the bits the oracle sees.  ``tags`` as in ``append``."""
+        device holds exactly the bits the oracle sees.  ``tags`` as in ``append``.  Not for an int8 index."""
+        if self.dtype != "bfloat16":
+            raise TypeError(f"append_bf16_bits needs a bfloat16 index; this one is {self.dtype}")
         bits = np.ascontiguousarray(bits, dtype=np.uint16)
-        assert bits.ndim == 2 and bits.shape[1] == self.dim
+        return self._append_in_place(torch.from_numpy(bits.view(np.int16)).view(torch.bfloat16), tags)
+
+    def _append_in_place(self, src, tags=None) -> int:
+        """Rows already of the index's element type (numpy or tensor [n, dim]) written into ``rows`` and committed."""
+        src = torch.from_numpy(np.ascontiguousarray(src)) if isinstance(src, np.ndarray) else src
+        assert src.dim() == 2 and src.shape[1] == self.dim and src.dtype == self.rows.dtype
         first = len(self)
-        n = bits.shape[0]
+        n = src.shape[0]
         if first + n > self.capacity:
-            raise capi.SaError(capi.SA_ERR_CAPACITY, "append_bf16_bits", "append past capacity")
-        src = torch.from_numpy(bits.view(np.int16)).view(torch.bfloat16)
+            raise capi.SaError(capi.SA_ERR_CAPACITY, "append", "append past capacity")
         self._write_tags(first, n, tags)
         self.rows[first:first + n].copy_(src)
         self.commit(first, n)
@@ -215,19 +247,23 @@ class VectorIndex:
 
     # ------------------------------------------------------------------ checkpoint / resume
     def snapshot(self, path: str) -> int:
-        """Write the committed rows (bf16 bits), their row terms, their filter tags and the similarity to ``path``
-        (.npz).  Returns the row count.
+        """Write the committed rows (bf16 bits, or int8), their row terms, their filter tags, the similarity and the
+        dtype to ``path`` (.npz).  Returns the row count.
         (The reference leaves corpus durability to Atlas; here a snapshot + the consumer-group offsets are the
         checkpoint, and replaying `documents_embed` from offset 0 is the fallback.)"""
         n = len(self)
         torch.cuda.current_stream(self.device).synchronize()
-        bits = self.rows[:n].view(torch.int16).cpu().numpy().view(np.uint16)
+        if self.dtype == "int8":
+            bits = self.rows[:n].cpu().numpy()
+        else:
+            bits = self.rows[:n].view(torch.int16).cpu().numpy().view(np.uint16)
         import os
         path = path if path.endswith(".npz") else path + ".npz"
         tmp = path + ".tmp"
         with open(tmp, "wb") as f:                       # written under a temporary name, then renamed: never half a file
             np.savez(f, rows=bits, inv_norm=self.inv_norm[:n].cpu().numpy(), dim=np.int64(self.dim),
-                     similarity=np.str_(self.similarity), tags=self.tags[:n].cpu().numpy().view(np.uint64))
+                     similarity=np.str_(self.similarity), tags=self.tags[:n].cpu().numpy().view(np.uint64),
+                     dtype=np.str_(self.dtype))
             f.flush()
             os.fsync(f.fileno())
         os.replace(tmp, path)
@@ -236,18 +272,25 @@ class VectorIndex:
     def restore(self, path: str) -> int:
         """Load a snapshot written by ``snapshot`` into this (empty or not) index, replacing its contents.  A snapshot
         without a recorded similarity is a cosine one; a snapshot of another similarity is refused (its row terms and
-        its rankings mean something else).  A snapshot without tags restores tag 0 on every row."""
+        its rankings mean something else).  A snapshot without tags restores tag 0 on every row.  Likewise a snapshot
+        that does not name a dtype is a bfloat16 one, and a snapshot of the other dtype is refused."""
         z = np.load(path if path.endswith(".npz") else path + ".npz")
         if int(z["dim"]) != self.dim:
             raise ValueError(f"snapshot has dim {int(z['dim'])}, index has {self.dim}")
         snap_sim = str(z["similarity"]) if "similarity" in z.files else "cosine"
         if snap_sim != self.similarity:
             raise ValueError(f"snapshot has similarity {snap_sim!r}, index has {self.similarity!r}")
+        snap_dtype = str(z["dtype"]) if "dtype" in z.files else "bfloat16"
+        if snap_dtype != self.dtype:
+            raise ValueError(f"snapshot has dtype {snap_dtype!r}, index has {self.dtype!r}")
         bits, inv = z["rows"], z["inv_norm"]
         n = bits.shape[0]
         if n > self.capacity:
             raise capi.SaError(capi.SA_ERR_CAPACITY, "restore", "snapshot larger than capacity")
-        self.rows[:n].copy_(torch.from_numpy(bits.view(np.int16)).view(torch.bfloat16))
+        if self.dtype == "int8":
+            self.rows[:n].copy_(torch.from_numpy(np.ascontiguousarray(bits, dtype=np.int8)))
+        else:
+            self.rows[:n].copy_(torch.from_numpy(bits.view(np.int16)).view(torch.bfloat16))
         self.inv_norm[:n].copy_(torch.from_numpy(inv))
         if "tags" in z.files:
             self.tags[:n].copy_(torch.from_numpy(np.ascontiguousarray(z["tags"], dtype=np.uint64).view(np.int64)))
@@ -273,14 +316,14 @@ class VectorIndex:
 
     # ------------------------------------------------------------------ search
     def search(self, q: torch.Tensor, k: int, want_score64: bool = False, filters=None):
-        """Device path.  q: [nq, dim] bf16 or fp32 CUDA tensor.  Returns (score f32 [nq,k], idx i32 [nq,k]
+        """Device path.  q: [nq, dim] CUDA tensor of the index's dtype (bf16 or int8) or fp32.  Returns (score f32 [nq,k], idx i32 [nq,k]
         [, score64 f64 [nq,k]]) as CUDA tensors, asynchronous on the current stream.  ``filters`` (uint64 [nq, 4] or
         [4], see ``filter_array``, or an int64 [nq, 4] tensor on q's device, see ``stage_filters``) restricts each query
         to the rows whose tag passes its filter."""
         assert q.is_cuda and q.dim() == 2 and q.shape[1] == self.dim
-        name = {torch.bfloat16: "sa_search", torch.float32: "sa_search_f32"}.get(q.dtype)
+        name = {self.rows.dtype: "sa_search", torch.float32: "sa_search_f32"}.get(q.dtype)
         if name is None:
-            raise TypeError("queries must be bf16 or fp32")
+            raise TypeError(f"queries of a {self.dtype} index must be {self.dtype} or fp32, not {q.dtype}")
         q = q.contiguous()
         nq = q.shape[0]
         dev = q.device
@@ -330,8 +373,9 @@ class VectorIndex:
 
     def search_hits(self, q: torch.Tensor, k: int, row_offset: int = 0, filters=None) -> torch.Tensor:
         """This shard's results in exchange format: uint8 CUDA tensor [nq, k, 16] = sa_hit {score f64, global row i64}
-        (``hits.view(torch.float64)[..., 0]`` / ``.view(torch.int64)[..., 1]``).  ``filters`` as in ``search``."""
-        assert q.is_cuda and q.dtype == torch.bfloat16 and q.dim() == 2 and q.shape[1] == self.dim
+        (``hits.view(torch.float64)[..., 0]`` / ``.view(torch.int64)[..., 1]``).  q: the index's dtype.  ``filters`` as
+        in ``search``."""
+        assert q.is_cuda and q.dtype == self.rows.dtype and q.dim() == 2 and q.shape[1] == self.dim
         q = q.contiguous()
         hits = torch.empty((q.shape[0], k, 16), dtype=torch.uint8, device=q.device)
         capi.search(self.lib, "sa_search_hits", self._h, q.data_ptr(), q.shape[0], k, int(row_offset), hits.data_ptr(),
@@ -386,7 +430,9 @@ class VectorIndex:
         return a.value, b.value, m.value
 
     def debug_tile_dots(self, q_bf16: torch.Tensor, tile: int, cta_group: int = 1) -> torch.Tensor:
-        """Test hook: raw Q.C^T accumulators of one 256-row corpus tile, [padded nq, 256] fp32."""
+        """Test hook: raw Q.C^T accumulators of one 256-row corpus tile, [padded nq, 256] fp32 (int8: the exact int32
+        accumulators rounded to fp32).  q: the index's dtype."""
+        assert q_bf16.dtype == self.rows.dtype
         nq = q_bf16.shape[0]
         rows = 128 * cta_group
         padded = (nq + rows - 1) // rows * rows

@@ -84,9 +84,14 @@ class ShardedIndex:
     def similarity(self) -> str:
         return getattr(self.index, "similarity", "cosine")
 
+    @property
+    def dtype(self) -> str:
+        """The element type of every rank's index ("bfloat16" for an index that does not say)."""
+        return getattr(self.index, "dtype", "bfloat16")
+
     # ------------------------------------------------------------------ device-resident queries
     def search(self, q: torch.Tensor, k: int, filters=None):
-        """q: [nq, dim] bf16 on this rank's device (identical on every rank).  Returns (score f32 [nq,k],
+        """q: [nq, dim] of the index's dtype (bf16 or int8) on this rank's device (identical on every rank).  Returns (score f32 [nq,k],
         global row i64 [nq,k]) -- the same on every rank.  ``filters`` (uint64 [nq, 4] or [4], the same on every rank)
         restricts each query to the rows whose tag passes its filter; each rank's index holds its own rows' tags."""
         nq = q.shape[0]
@@ -136,7 +141,11 @@ class ShardedIndex:
 
     def _search_host_blocking(self, q: np.ndarray, k: int, filters=None):
         dev = self.index.rows.device if hasattr(self.index, "rows") else torch.device("cpu")
-        qd = torch.from_numpy(q).to(dev).to(torch.bfloat16)
+        if self.dtype == "int8":
+            from .engine import int8_round
+            qd = torch.from_numpy(int8_round(q)).to(dev)
+        else:
+            qd = torch.from_numpy(q).to(dev).to(torch.bfloat16)
         s, gi = self.search(qd, k, filters=filters)
         return s.cpu().numpy(), gi.cpu().numpy()
 
@@ -155,10 +164,11 @@ class MultiGpuIndex:
     ``reset``, ``__len__``, ``search_host[_submit/_wait]``) with DENSE row ids in append order; inside, append batches go
     round-robin to the shards (SURVEY.md section 8e: "append-only streams go round-robin by epoch") and the library's
     global rows (shard * capacity + local row) are translated back through a per-shard table.  ``max_k`` (at most 64,
-    ``capi.SA_MAX_K``) is the largest k of a search on every shard."""
+    ``capi.SA_MAX_K``) is the largest k of a search on every shard; ``similarity`` and ``dtype`` ("bfloat16" or "int8",
+    see ``VectorIndex``) are those of every shard."""
 
     def __init__(self, dim: int, capacity_per_gpu: int, max_batch: int, max_k: int, n_gpus: int | None = None,
-                 similarity: str = "cosine"):
+                 similarity: str = "cosine", dtype: str = "bfloat16"):
         from .engine import VectorIndex
         n = torch.cuda.device_count() if n_gpus is None else int(n_gpus)
         if n < 1 or n > torch.cuda.device_count():
@@ -166,8 +176,9 @@ class MultiGpuIndex:
         self.n = n
         self.dim, self.capacity_per_gpu = dim, int(capacity_per_gpu)
         self.similarity = similarity
+        self.dtype = dtype
         self.shards = [VectorIndex(dim=dim, capacity=capacity_per_gpu, max_batch=max_batch, max_k=max_k, device=g,
-                                   similarity=similarity) for g in range(n)]
+                                   similarity=similarity, dtype=dtype) for g in range(n)]
         self.lib = self.shards[0].lib
         path = capi.bundled_nccl_path()
         if path:
@@ -201,9 +212,10 @@ class MultiGpuIndex:
         self._next = 0
 
     def append(self, rows_f32: np.ndarray, tags=None) -> int:
-        """Append a batch of fp32 embeddings to the next shard (round-robin).  Returns the first (dense) row id.
-        ``tags`` (uint64 [n]) are the rows' filter tags (0 without)."""
-        rows_f32 = np.ascontiguousarray(rows_f32, dtype=np.float32)
+        """Append a batch of fp32 embeddings (int8 ones too, for an int8 index) to the next shard (round-robin).  Returns
+        the first (dense) row id.  ``tags`` (uint64 [n]) are the rows' filter tags (0 without)."""
+        rows_f32 = np.asarray(rows_f32)
+        rows_f32 = np.ascontiguousarray(rows_f32, dtype=np.int8 if rows_f32.dtype == np.int8 else np.float32)
         first = len(self._where)
         if len(rows_f32) == 0:
             return first
