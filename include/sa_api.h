@@ -63,6 +63,9 @@ typedef enum sa_status {
 /* Largest k of a search.  Candidate lists hold 16 (k <= 16) or 32 entries per tile lane; a "deep" search (28 < k <= 64)
  * keeps the 32-entry lists and runs a scan variant whose shared bounds hold for its k (DESIGN.md section 4.1). */
 #define SA_MAX_K 64
+/* Largest dim of either element type: the exact fallback scan stages one query row (2 SA_MAX_DIM bytes of bf16) in
+ * shared memory, and an int8 |<q,c>| <= dim 2^14 stays inside the int32 accumulators. */
+#define SA_MAX_DIM 65536
 #define SA_HOST_SLOTS 2 /* host-buffer searches that may be in flight at once (sa_search_host_submit) */
 
 int sa_version(void);
@@ -75,11 +78,11 @@ const char* sa_last_error(void); /* thread-local detail of the last failure on t
  *   'mongodb.index'='vector_index', 'mongodb.embedding_column'='embedding', ...)
  *   (terraform/lab2-vector-search/main.tf:215) and the index definition {numDimensions 1536, similarity cosine}
  *   (assets/pre-setup/MongoDB-Setup.md:72-83, scripts/common/validate.py:56-61,167-180).
- * dim must be a multiple of 64 (1536 and 768 are); capacity_rows < 2^31; max_k <= SA_MAX_K.  sa_engine_create makes a
- * cosine index; sa_engine_create_sim takes the similarity (SA_SIM_*) and rejects any other value with SA_ERR_ARG before
- * it touches a device.  sa_engine_create_elem also takes the element type (SA_ELEM_*; sa_engine_create_sim is it with
- * SA_ELEM_BF16); an int8 index needs dim to be a multiple of 128 and at most 65536 (so |<q,c>| <= dim 2^14 fits in
- * int32).  An unknown elem or such a dim is rejected with SA_ERR_ARG before it touches a device. */
+ * dim must be a multiple of 64 (1536 and 768 are) and at most SA_MAX_DIM; capacity_rows < 2^31; max_k <= SA_MAX_K.
+ * sa_engine_create makes a cosine index; sa_engine_create_sim takes the similarity (SA_SIM_*) and rejects any other value
+ * with SA_ERR_ARG before it touches a device.  sa_engine_create_elem also takes the element type (SA_ELEM_*;
+ * sa_engine_create_sim is it with SA_ELEM_BF16); an int8 index needs dim to be a multiple of 128.  An unknown elem or
+ * such a dim (of either type) is rejected with SA_ERR_ARG before it touches a device. */
 int sa_engine_create(sa_engine** out, int device, int dim, int64_t capacity_rows, int max_batch, int max_k);
 int sa_engine_create_sim(sa_engine** out, int device, int dim, int64_t capacity_rows, int max_batch, int max_k,
                          int similarity);
@@ -93,6 +96,8 @@ void sa_engine_destroy(sa_engine* e);
  *   cosine      1/|c| over the stored values (int8: rounded once from fp64), 0 for an all-zero row or a tombstone
  *   dotProduct  1 for a live row, 0 for a tombstone
  *   euclidean   |c|^2/2 (summed in fp64, rounded once to fp32) for a live row, negative (e.g. -1) for a tombstone
+ * A bf16 row holding a NaN or an infinite element is not live under any similarity: ingest gives it the tombstone term
+ * (cosine 0, dotProduct 0, euclidean -1), it never enters the norm bound below, and no search returns it.
  * The ingest entry points below write it; a caller that tombstones a row writes the row's term itself (and may zero the
  * row).  n_valid rows are taken as already committed (their terms valid); for dotProduct and euclidean the bound on the
  * rows' norms that the search's certificate uses is recomputed over them. */

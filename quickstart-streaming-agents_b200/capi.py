@@ -18,6 +18,7 @@ SA_ERR_COMM = -3
 SA_ERR_CAPACITY = -4
 SA_ERR_DEVICE = -5
 SA_MAX_K = 64   # deep searches (28 < k <= 64) keep 32-entry lists with bounds valid for their k
+SA_MAX_DIM = 65536   # largest dim of either element type
 SA_HOST_SLOTS = 2
 SA_COMM_ID_BYTES = 128
 SA_SIM_COSINE = 0

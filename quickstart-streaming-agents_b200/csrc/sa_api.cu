@@ -665,11 +665,8 @@ int do_search(sa_engine* e, const void* q_dev, int nq, int k, float* out_score, 
     fp.zero_c_n = e->opt_window_bound ? static_cast<int>(plan.size()) * e->num_sms * 128 : 0;
     fp.row_tags = filters != nullptr ? e->row_tags : nullptr;
     fp.filters = filters;
-    // the query in shared memory: as fp32 (bf16), or its bytes (int8)
-    const size_t smem = e->elem == SA_ELEM_INT8 ? row_bytes : static_cast<size_t>(e->dim) * sizeof(float);
-    if (smem > 48 * 1024)
-      SA_CUDA(cudaFuncSetAttribute(sa::sa_fixup_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-    sa::sa_fixup_kernel<<<2 * e->num_sms, sa::kFixThreads, smem, st>>>(fp);
+    // the query's bytes in shared memory (the kernel's limit was raised for SA_MAX_DIM at engine creation)
+    sa::sa_fixup_kernel<<<2 * e->num_sms, sa::kFixThreads, row_bytes, st>>>(fp);
     SA_CUDA(cudaGetLastError());
     tm.kernels += 1;
     e->scratch_dirty = false;
@@ -724,6 +721,7 @@ static_assert(sizeof(sa_filter) == sizeof(sa::Filter) && offsetof(sa_filter, all
               "sa_filter and sa::Filter must share one layout");
 static_assert(SA_MAX_K == sa::kDeepMaxK && sa::kFixMaxK >= SA_MAX_K && sa::kShallowMaxK < SA_MAX_K,
               "every k <= SA_MAX_K has a scan variant and fits the fallback's lists");
+static_assert(sa::kFixSmemMax == 2 * SA_MAX_DIM, "the fallback's shared memory holds one bf16 query of SA_MAX_DIM");
 
 int sa_version(void) { return 100; }
 
@@ -759,9 +757,11 @@ int sa_engine_create_elem(sa_engine** out, int device, int dim, int64_t capacity
   if (elem != SA_ELEM_BF16 && elem != SA_ELEM_INT8)
     return fail(SA_ERR_ARG, "elem %d is not SA_ELEM_BF16 (0) or SA_ELEM_INT8 (1)", elem);
   if (dim <= 0 || dim % 64 != 0) return fail(SA_ERR_ARG, "dim %d must be a positive multiple of 64", dim);
-  // int8: a K slice is 128 elements, and |<q,c>| <= dim 2^14 must stay inside the int32 accumulators
-  if (elem == SA_ELEM_INT8 && (dim % 128 != 0 || dim > 65536))
-    return fail(SA_ERR_ARG, "an int8 index needs dim %d to be a multiple of 128 and at most 65536", dim);
+  // the fallback scan stages one query row in shared memory; int8: |<q,c>| <= dim 2^14 stays inside int32
+  if (dim > SA_MAX_DIM) return fail(SA_ERR_ARG, "dim %d must be at most %d (SA_MAX_DIM)", dim, SA_MAX_DIM);
+  // int8: a K slice is 128 elements
+  if (elem == SA_ELEM_INT8 && dim % 128 != 0)
+    return fail(SA_ERR_ARG, "an int8 index needs dim %d to be a multiple of 128", dim);
   if (capacity_rows <= 0 || capacity_rows >= (1ll << 31) - 512)
     return fail(SA_ERR_ARG, "capacity_rows %lld outside (0, 2^31-512)", (long long)capacity_rows);
   if (max_batch <= 0) return fail(SA_ERR_ARG, "max_batch must be positive");
@@ -776,6 +776,9 @@ int sa_engine_create_elem(sa_engine** out, int device, int dim, int64_t capacity
                 prop.minor);
   SA_ON_DEVICE(device);
   if (!get_encode_fn()) return fail(SA_ERR_CUDA, "cuTensorMapEncodeTiled entry point not available");
+  // The fallback scan's dynamic shared memory is one query row, 2 SA_MAX_DIM bytes at most: the kernel's limit is set
+  // once for that size on this device, so searches of engines with different dims never set it concurrently.
+  SA_CUDA(cudaFuncSetAttribute(sa::sa_fixup_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, sa::kFixSmemMax));
 
   sa_engine* e = new sa_engine();
   e->device = device;

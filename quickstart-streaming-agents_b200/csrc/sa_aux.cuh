@@ -86,14 +86,19 @@ constexpr int kElemBf16 = 0;
 constexpr int kElemI8 = 1;
 __host__ __device__ __forceinline__ int elem_bytes(int elem) { return elem == kElemI8 ? 1 : 2; }
 
-// Row term of a live row from its float64 sum of squares (dotProduct, euclidean); cosine keeps its fp32 path below.
+// Row term of a row from its float64 sum of squares (dotProduct, euclidean); cosine keeps its fp32 path below.
 // |c|^2 is summed in fp64 and rounded once: an fp32 sum of 1536 squares is off by ~1e-4 relative, the size of the whole
-// certificate band.  Also returns (through cmax) an upper bound on the row's norm: sqrt in fp64, nudged up, rounded up.
+// certificate band.  The fp64 sum of squares of bf16 values cannot overflow, so a non-finite sum means a NaN or inf
+// element: such a row gets the tombstone term and is never returned, as under cosine and in the definition.
 template <int kSim>
 __device__ __forceinline__ float row_term_f64(double ss) {
+  if (!isfinite(ss)) return kSim == kSimEuc ? -1.0f : 0.0f;
   return kSim == kSimEuc ? __double2float_rn(0.5 * ss) : 1.0f;
 }
+// An upper bound on the row's norm for Cmax: sqrt in fp64, nudged up, rounded up.  0 (no contribution) for a row that
+// row_term_f64 tombstones.
 __device__ __forceinline__ unsigned norm_bound_bits(double ss) {
+  if (!isfinite(ss)) return 0u;
   return __float_as_uint(__double2float_ru(sqrt(ss) * (1.0 + 0x1p-40)));
 }
 // Raise the device scalar Cmax (float bits; non-negative floats order like their bits) by the largest bound of a block.
@@ -128,7 +133,12 @@ __global__ void sa_rownorm_kernel(const uint16_t* __restrict__ rows, float* __re
   if (lane == 0) inv_norm[first + w] = ss > 0.f ? 1.0f / sqrtf(ss) : 0.f;
 }
 
-// fp64 sum of squares of one bf16 row (squares of bf16 values are exact in fp32), one warp, every lane gets it.
+// Square of a bf16 value in fp64: exact, and finite for every finite value (an fp32 square overflows past 2^64).
+__device__ __forceinline__ double sq_f64(float a) {
+  const double d = static_cast<double>(a);
+  return d * d;
+}
+// fp64 sum of squares of one bf16 row, one warp, every lane gets it.
 __device__ __forceinline__ double row_ss_f64(const uint4* __restrict__ src, int nvec, int lane) {
   double ss = 0.0;
   for (int i = lane; i < nvec; i += 32) {
@@ -136,9 +146,8 @@ __device__ __forceinline__ double row_ss_f64(const uint4* __restrict__ src, int 
     const uint32_t u[4] = {x.x, x.y, x.z, x.w};
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
-      const float a = bf16_bits_to_f32(u[k] & 0xffffu), b = bf16_bits_to_f32(u[k] >> 16);
-      ss += static_cast<double>(a * a);
-      ss += static_cast<double>(b * b);
+      ss += sq_f64(bf16_bits_to_f32(u[k] & 0xffffu));
+      ss += sq_f64(bf16_bits_to_f32(u[k] >> 16));
     }
   }
   return warp_sum(ss);
@@ -210,10 +219,10 @@ __global__ void sa_convert_rows_term_kernel(const float* __restrict__ src, uint1
       d[i] = make_uint2(b0 | (b1 << 16), b2 | (b3 << 16));
       const float r0 = bf16_bits_to_f32(b0), r1 = bf16_bits_to_f32(b1), r2 = bf16_bits_to_f32(b2),
                   r3 = bf16_bits_to_f32(b3);
-      ss += static_cast<double>(r0 * r0);
-      ss += static_cast<double>(r1 * r1);
-      ss += static_cast<double>(r2 * r2);
-      ss += static_cast<double>(r3 * r3);
+      ss += sq_f64(r0);
+      ss += sq_f64(r1);
+      ss += sq_f64(r2);
+      ss += sq_f64(r3);
     }
     ss = warp_sum(ss);
     if (lane == 0) w_out[w] = row_term_f64<kSim>(ss);
@@ -622,7 +631,7 @@ __global__ void __launch_bounds__(kMergeThreads) sa_merge_rescore_kernel(const M
 // Always launched; with an empty work queue (the normal case) it only converts the internal result to the caller's
 // output arrays and re-zeroes the scan's scratch for the next search.
 //
-// Work item = (queue entry, chunk of kFixChunkTiles tiles of that lane).  A CTA stages the query (fp32) in shared memory;
+// Work item = (queue entry, chunk of kFixChunkTiles tiles of that lane).  A CTA stages the query's bytes in shared memory;
 // each warp walks rows: fp32 dot (CUDA cores) * w (euclidean: - w) -> a'(r), whose error is inside eps; rows with a' >=
 // max(band, current k-th exact value in approximate units - eps) are re-scored exactly and inserted into the WARP's own list (no
 // sharing between warps, so no locks in shared memory); at the end of the item one thread folds the warps' lists into the
@@ -670,6 +679,7 @@ struct FixParams {
 constexpr int kFixThreads = 256;
 constexpr int kFixChunkTiles = 8;
 constexpr int kFixMaxK = 64;  // per-warp lists of k <= 64 entries in shared memory (SA_MAX_K)
+constexpr int kFixSmemMax = 2 * 65536;  // dynamic shared memory: one bf16 query row of SA_MAX_DIM elements
 
 __device__ __forceinline__ void fix_finalize(const FixParams& p, int first, int stride) {
   const int total = p.nq * p.k;
@@ -710,8 +720,7 @@ __device__ __forceinline__ void fix_list_insert(D* cosv, I* rowv, int k, double 
 }
 
 __global__ void __launch_bounds__(kFixThreads) sa_fixup_kernel(const FixParams p) {
-  extern __shared__ float4 fix_smem[];  // bf16 query as fp32: [dim/8] float4 "lo" halves, then [dim/8] "hi" halves;
-                                        // int8 query: its dim bytes as they are
+  extern __shared__ uint4 q_s[];  // the query's row bytes as they are (bf16 or int8): at most 2 SA_MAX_DIM bytes
   constexpr int kWarps = kFixThreads / 32;
   __shared__ double l_cos[kWarps][kFixMaxK];  // one list per warp, touched by that warp's lane 0 only
   __shared__ int l_row[kWarps][kFixMaxK];
@@ -728,9 +737,6 @@ __global__ void __launch_bounds__(kFixThreads) sa_fixup_kernel(const FixParams p
   const bool i8 = p.elem == kElemI8;
   const size_t row_bytes = static_cast<size_t>(p.dim) * elem_bytes(p.elem);
   const int nvec = static_cast<int>(row_bytes / 16);
-  float4* q_lo = fix_smem;
-  float4* q_hi = fix_smem + nvec;
-  const uint4* q_i8 = reinterpret_cast<const uint4*>(fix_smem);
   const long long items = static_cast<long long>(count) * p.chunks_per_entry;
   for (long long item = blockIdx.x; item < items; item += gridDim.x) {
     const FixEntry en = p.entries[item / p.chunks_per_entry];
@@ -748,17 +754,7 @@ __global__ void __launch_bounds__(kFixThreads) sa_fixup_kernel(const FixParams p
     if (p.filters != nullptr) flt = p.filters[en.q];
 
     __syncthreads();  // previous item's smem no longer in use
-    for (int i = tid; i < nvec; i += kFixThreads) {
-      const uint4 x = __ldg(qv + i);
-      if (i8) {
-        reinterpret_cast<uint4*>(fix_smem)[i] = x;
-        continue;
-      }
-      q_lo[i] = make_float4(bf16_bits_to_f32(x.x & 0xffffu), bf16_bits_to_f32(x.x >> 16), bf16_bits_to_f32(x.y & 0xffffu),
-                            bf16_bits_to_f32(x.y >> 16));
-      q_hi[i] = make_float4(bf16_bits_to_f32(x.z & 0xffffu), bf16_bits_to_f32(x.z >> 16), bf16_bits_to_f32(x.w & 0xffffu),
-                            bf16_bits_to_f32(x.w >> 16));
-    }
+    for (int i = tid; i < nvec; i += kFixThreads) q_s[i] = __ldg(qv + i);
     for (int i = tid; i < kWarps * kFixMaxK; i += kFixThreads) {
       l_cos[i / kFixMaxK][i % kFixMaxK] = -INFINITY;
       l_row[i / kFixMaxK][i % kFixMaxK] = -1;
@@ -791,23 +787,23 @@ __global__ void __launch_bounds__(kFixThreads) sa_fixup_kernel(const FixParams p
           int iacc = 0;
           for (int i = lane; i < nvec; i += 32) {
             const uint4 y = __ldg(cv + i);
-            const uint4 x = q_i8[i];
+            const uint4 x = q_s[i];
             iacc = dp4a_s8(x.x, y.x, dp4a_s8(x.y, y.y, dp4a_s8(x.z, y.z, dp4a_s8(x.w, y.w, iacc))));
           }
           acc = __int2float_rn(warp_sum(iacc));
         } else {
+          // both operands widened from their bits (bf16 -> fp32 is exact)
           acc = 0.f;
           for (int i = lane; i < nvec; i += 32) {
             const uint4 y = __ldg(cv + i);
-            const float4 a = q_lo[i], b = q_hi[i];
-            acc = fmaf(a.x, bf16_bits_to_f32(y.x & 0xffffu), acc);
-            acc = fmaf(a.y, bf16_bits_to_f32(y.x >> 16), acc);
-            acc = fmaf(a.z, bf16_bits_to_f32(y.y & 0xffffu), acc);
-            acc = fmaf(a.w, bf16_bits_to_f32(y.y >> 16), acc);
-            acc = fmaf(b.x, bf16_bits_to_f32(y.z & 0xffffu), acc);
-            acc = fmaf(b.y, bf16_bits_to_f32(y.z >> 16), acc);
-            acc = fmaf(b.z, bf16_bits_to_f32(y.w & 0xffffu), acc);
-            acc = fmaf(b.w, bf16_bits_to_f32(y.w >> 16), acc);
+            const uint4 x = q_s[i];
+            const uint32_t u[4] = {x.x, x.y, x.z, x.w};
+            const uint32_t v[4] = {y.x, y.y, y.z, y.w};
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+              acc = fmaf(bf16_bits_to_f32(u[k] & 0xffffu), bf16_bits_to_f32(v[k] & 0xffffu), acc);
+              acc = fmaf(bf16_bits_to_f32(u[k] >> 16), bf16_bits_to_f32(v[k] >> 16), acc);
+            }
           }
           acc = warp_sum(acc);
         }

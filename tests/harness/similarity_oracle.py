@@ -8,7 +8,9 @@ keeps its own definition there, and this module reuses its bf16 helpers.
                   dotProduct  <q,c>
                   euclidean   d = sqrt(max(0, (|q|^2 - 2 <q,c>) + |c|^2))   -- the engine's formula, term for term
     result        the k best rows: (value desc, row asc), for euclidean (d asc, row asc);
-                  rows with live[r] False (tombstones) are never returned; empty slots hold (-inf, -1), (+inf, -1) for d
+                  rows with live[r] False (tombstones) are never returned, nor is a row whose value is not finite (a
+                  row holding a NaN or inf element, under every similarity); empty slots hold (-inf, -1), (+inf, -1)
+                  for d
 
 All arithmetic runs over the bf16-rounded values with float64 sums.  bf16 x bf16 products have at most 16 significant
 bits, so the sums are exact for any data whose magnitudes span less than ~2^30 within a row, and the summation order
@@ -56,6 +58,7 @@ class RunningTopk:
         m = s.shape[1]
         if m == 0:
             return
+        s = np.where(np.isfinite(s), s, -np.inf)     # a NaN would sort last in the partition below and hide a row
         kk = min(self.k, m)
         kth = np.partition(s, m - kk, axis=1)[:, m - kk]
         for r in range(s.shape[0]):

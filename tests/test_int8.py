@@ -33,6 +33,7 @@ def create(lib, dim, elem, sim=capi.SA_SIM_COSINE):
     (256, 2, b"elem 2"), (256, -1, b"elem -1"),                                  # unknown element types
     (64, capi.SA_ELEM_INT8, b"multiple of 128"), (192, capi.SA_ELEM_INT8, b"multiple of 128"),
     (65664, capi.SA_ELEM_INT8, b"at most 65536"),                               # |<q,c>| would leave int32
+    (65600, capi.SA_ELEM_BF16, b"at most 65536"),         # the fallback scan's query row would not fit shared memory
 ])
 def test_create_elem_refuses_before_touching_a_device(lib, dim, elem, what):
     rc, h = create(lib, dim, elem)
